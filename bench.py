@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's metric on BASELINE.json's config, measured on B200.
+"""bench.py -- BASELINE.json's metric on BASELINE.json's config, measured on an H100.
 
 Metric: Mrays/s (whole job) for full-image renders of the synthetic "lego_render" scene (BASELINE configs[1]:
 800x800 = 640,000 rays per image, K=8, N=400,000 neural points, SR=24 shading samples per ray, D=400 march steps, fp32 I/O).
 A "step" = one full image per GPU through the hot path (voxel query -> row packing -> fused pair MLPs -> colour MLP ->
 composite), ONE `render_full` call.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--sr 24] [--only main]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--sr 24] [--only main] [--dump-outputs DIR]
 
 N>1 is launched by torchrun (one rank per GPU, NCCL).  The JSON line of every N carries
   value / ms_per_step  WEAK scaling: N distinct camera poses (rolls about the view axis), rank g renders frame g, one all-gather of
@@ -18,6 +18,11 @@ N>1 is launched by torchrun (one rank per GPU, NCCL).  The JSON line of every N 
   scannet              BASELINE configs[4]: N=5M points (P=30), the same step with the sparse touched-rows gradient exchange, plus one
                        prune + probe + grow cycle (variable-length all-gather of the new points);
   cold, sr80           (N=1) first frame of a new point cloud (voxel grid + per-point table built inside the timed region); SR=80.
+
+`--dump-outputs DIR` writes what the timed path computed in its last timed step (the arrays a caller of render_full receives) as
+DIR/<name>.npy (float32): coarse_raycolor, coarse_is_background and ray_mask of the whole frame, coarse_point_opacity of a fixed seeded
+sample of 131,072 rays (their indices in coarse_point_opacity_rays.npy).  The inputs are seeded: equal arguments give equal inputs, so two
+builds can be compared output for output.
 
 `--impl reference` times the reference's own CPU path (the oracle port: oracle/query_oracle.c + oracle/shade_oracle.py, i.e. the
 reference's algorithm on the host cores) on a bounded, stratified sample of the same frame.  The oracle is used here ONLY as the
@@ -44,11 +49,11 @@ METRIC = "Mrays/s (800x800 render, K=8, 400k pts, SR=24), whole job"
 FLOPS_PER_PAIR = 542720.0    # SURVEY.md 8(d): 2*(284*256 + 256*256 + 263*256 + 256*256 + 256)
 FLOPS_PER_SAMPLE = 137984.0  # 2*(280*128 + 128*128 + 128*128 + 128*3)
 # kernels of libpnb200.so launched per render_full (memsets / torch fills are not counted): march, 2 scans x 3, expand, knn, valid_list,
-# count_rays (query = 11); k_pack_quads, k_pack_scan, k_pack_place, pair kernel, colour kernel (tcgen05 shading = 5); composite (1)
+# count_rays (query = 11); k_pack_quads, k_pack_scan, k_pack_place, pair kernel, colour kernel (wgmma shading = 5); composite (1)
 LAUNCHES_PER_STEP_TC = 11 + 5 + 1
 LAUNCHES_PER_STEP_FP32 = 11 + 1 + 1
-MMA_FLOPS = 2.0 * 128 * 256 * 16                      # one tcgen05.mma M128 N256 K16
-MMAS_PER_TILE = {True: 159, False: 201}               # frozen (k_shade_tc8) / general (k_shade_tc7) pair kernel, per 128-row tile
+MMA_FLOPS = 2.0 * 128 * 256 * 16                      # one K = 16 product of a 128 x 256 tile (two wgmma m64n256k16)
+MMAS_PER_TILE = {True: 159, False: 201}               # frozen / general k_shade_wg, per 128-row tile: K = 16 steps x 3 (BF16x3)
 
 
 def peaks():
@@ -57,7 +62,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained"),
                     source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=None, source="H100 SXM data sheet (dense)")
 
 
 class ClockSampler:
@@ -302,9 +307,10 @@ def time_region(D, flush, fn, steps):
     return D.max_over_ranks(e0.elapsed_time(e1))
 
 
-def render_section(D, net, cam_list, rays_host, steps, warmup, flush, e2e=False):
+def render_section(D, net, cam_list, rays_host, steps, warmup, flush, e2e=False, last=None):
     """Times `steps` frames.  rays_host: this rank's pinned [R,3] ray directions; cam_list: (campos, camrot, near, far, bg).
-    Resident mode: rays already on the device.  e2e mode: H2D of the rays and D2H of the colours inside every step."""
+    Resident mode: rays already on the device.  e2e mode: H2D of the rays and D2H of the colours inside every step.
+    last: a dict that receives the render_full outputs of the last step."""
     dev = D.dev
     R = rays_host.shape[0]
     rays_dev = rays_host.to(dev)
@@ -316,6 +322,9 @@ def render_section(D, net, cam_list, rays_host, steps, warmup, flush, e2e=False)
         with torch.no_grad():
             out = net.render_full(cam_list[0], rd, cam_list[1], cam_list[2], cam_list[3], cam_list[4])
         col = out["coarse_raycolor"][0]
+        if last is not None:
+            last.clear()
+            last.update(out)
         if D.world > 1:
             D.gather_async(col, gathered[k & 1])
         if e2e:
@@ -338,6 +347,22 @@ def render_section(D, net, cam_list, rays_host, steps, warmup, flush, e2e=False)
     return ms, R
 
 
+DUMP_SAMPLE_RAYS = 131072
+
+
+def dump_outputs(out_dir, out):
+    """The arrays render_full returned in the last timed step -> out_dir/<name>.npy (float32, < 64 MB in all): the per-ray outputs of the
+    whole frame, the per-sample opacities [R, SR] of a fixed seeded sample of rays (the whole [R, SR] array is 61 MB at SR = 24)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for k in ("coarse_raycolor", "coarse_is_background", "ray_mask"):
+        np.save(os.path.join(out_dir, k + ".npy"), out[k][0].float().cpu().numpy())
+    op = out["coarse_point_opacity"][0]
+    R = op.shape[0]
+    rays = np.sort(np.random.RandomState(0).choice(R, size=min(DUMP_SAMPLE_RAYS, R), replace=False))
+    np.save(os.path.join(out_dir, "coarse_point_opacity.npy"), op[torch.from_numpy(rays).to(op.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "coarse_point_opacity_rays.npy"), rays.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -347,8 +372,9 @@ def main():
     ap.add_argument("--sr", type=int, default=24)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--only", type=str, default="", help="comma list of sub-results to run besides the main line: strong,truck,train,scannet,cold,sr80 (default: all)")
-    ap.add_argument("--precision", type=str, default="bf16x3", help="bf16x3 (tcgen05, default) | fp32 (CUDA cores)")
-    ap.add_argument("--frozen", type=int, default=1, help="1 (default): frozen-cloud pair kernel k_shade_tc8 (point-only layer-1 inputs hoisted per point) | 0: general kernel k_shade_tc7")
+    ap.add_argument("--precision", type=str, default="bf16x3", help="bf16x3 (wgmma, default) | fp32 (CUDA cores)")
+    ap.add_argument("--frozen", type=int, default=1, help="1 (default): frozen-cloud pair kernel (point-only layer-1 inputs hoisted per point) | 0: general pair kernel")
+    ap.add_argument("--dump-outputs", type=str, default="", metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)
@@ -363,7 +389,7 @@ def main():
     rank, world = D.rank, D.world
     assert world == args.gpus, "WORLD_SIZE %d != --gpus %d (launch N>1 with torchrun)" % (world, args.gpus)
     W = max(args.warmup, 3)
-    flush = torch.empty(160 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(160 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     cfg = scene.CONFIGS["lego_render"]
     cfg.SR = args.sr
@@ -384,10 +410,13 @@ def main():
     # share their host, and a stalled launching thread occasionally adds milliseconds to a region that has nothing to do with the GPU
     # work - the repeat makes such a run recognisable
     regions = []
-    for _ in range(2):
+    for i in range(2):
         t_w0 = time.time()
-        ms_i, R = render_section(D, net, cam, mine, args.steps, 0, flush)
+        last = {} if i == 0 else None
+        ms_i, R = render_section(D, net, cam, mine, args.steps, 0, flush, last=last)
         regions.append((ms_i, t_w0, time.time()))
+        if last and args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last)
     ms_res, t_w0, t_w1 = regions[0]
     clocks = sampler.stop(t_w0, t_w1) if sampler else None
     # workload counters (oracle-independent: the library's own device counters)
@@ -440,10 +469,10 @@ def main():
                        "pnb_shade_forward_tc")
         shade_avg = time_kernel(lambda: tc(_lib.TC_PAIRS))
         color_avg = time_kernel(lambda: tc(_lib.TC_COLOR))
-        kname = ("k_shade_tc8 (frozen cloud: the 224 point-only inputs of block1.0 hoisted into a per-point table)" if frozen else "k_shade_tc7") + \
-            " incl. the 3 row-packing kernels (tcgen05 BF16x3 pair MLPs 284-256-256 | 263-256-256 + alpha + K-reduction)"
+        kname = ("k_shade_wg<FROZEN> (frozen cloud: the 224 point-only inputs of block1.0 hoisted into a per-point table)" if frozen else "k_shade_wg") + \
+            " incl. the 3 row-packing kernels (wgmma BF16x3 pair MLPs 284-256-256 | 263-256-256 + alpha + K-reduction)"
         kflops = FLOPS_PER_PAIR * qc["n_pairs"]
-        n_tiles = math.ceil(qc["n_pairs"] / 0.993 / 128.0)       # packed rows: 99.3 % fill (tools/tc_profile.py prints the exact count)
+        n_tiles = math.ceil(qc["n_pairs"] / 0.993 / 128.0)       # packed rows: 99.3 % fill on the lego frame
         issued = MMAS_PER_TILE[frozen] * MMA_FLOPS * n_tiles
         n_launch = LAUNCHES_PER_STEP_TC
         net.check_errors()
@@ -455,10 +484,6 @@ def main():
     value = total_rays / (ms_res * 1e-3) / 1e6
     e2e_val = total_rays / (ms_e2e * 1e-3) / 1e6
     pk = peaks()
-    traffic = None
-    tfile = os.path.join(ROOT, "profiles", "r02_ncu_dram_traffic.json")
-    if os.path.exists(tfile) and args.precision != "fp32" and args.sr == 24:
-        traffic = json.load(open(tfile)).get("k_shade_tc8" if frozen else "k_shade_tc7", None)
     achieved = kflops / (shade_avg * 1e-3) / 1e12
     peak = pk["bf16_tflops"]
 
@@ -524,7 +549,7 @@ def main():
         line = dict(
             metric=METRIC, value=value, unit="Mrays/s", n_gpus=world, steps=args.steps, warmup=W,
             ms_per_step=ms_res / args.steps, higher_is_better=True, scaling="weak", vs_baseline=None,
-            dtype=("f32 (bf16x3 split on tcgen05, fp32 accumulate)" if args.precision != "fp32" else "f32"),
+            dtype=("f32 (bf16x3 split on wgmma, fp32 accumulate)" if args.precision != "fp32" else "f32"),
             data="synthetic",
             config=dict(workload=WORKLOAD % args.sr,
                         rays_per_step_per_gpu=R,
@@ -533,7 +558,7 @@ def main():
                         parallelism=("%d distinct poses (rolls about the view axis), rank g renders frame g; points / grid / MLP replicated%s"
                                      % (world, "; one all-gather of the colours per step on a side stream" if world > 1 else "")),
                         l2="flushed before every timed step (160 MiB fill inside the region); the per-frame working set (410 MB per-point "
-                           "table, 3.5 GB h-bar) exceeds the 126 MB L2 anyway",
+                           "table, 3.5 GB h-bar) exceeds the 50 MB L2 anyway",
                         workload_counters=dict(hit_rays=qc["R2"], valid_samples=qc["n_valid"], valid_pairs=qc["n_pairs"],
                                                candidate_samples=qc["n_cand"], occupied_voxels=gc["n_occ"], max_pts_per_voxel=gc["max_pts"])),
             e2e=dict(value=e2e_val, unit="Mrays/s", h2d_bytes_per_step=int(mine.numel() * 4 * world),
@@ -541,13 +566,13 @@ def main():
             gpu_launches=n_launch * args.steps,
             clocks=clocks,
             roofline=dict(bound="tensor", kernel=kname, achieved=achieved, peak=peak, unit="TFLOP/s",
-                          frac=achieved / peak, traffic=traffic, peak_source="%s bf16 cuBLAS burst (MEASURED_PEAKS.json)" % pk["source"],
+                          frac=achieved / peak, peak_source=pk["source"],
                           algorithmic_flops_per_launch=kflops, kernel_ms=shade_avg,
                           kernel_share_of_step=shade_avg / (ms_res / args.steps),
                           issued_mma_flops_per_launch=issued,
                           tensor_pipe_frac_issued=(issued / (shade_avg * 1e-3) / 1e12 / peak if issued else None),
                           note=("algorithmic = SURVEY 8(d) formula (542,720 FLOP per valid pair); the frozen pipeline computes 21 % of "
-                                "them once per point instead of once per pair, issued = the tcgen05.mma actually launched (BF16x3: 3 per product)"
+                                "them once per point instead of once per pair, issued = the wgmma actually launched (BF16x3: 3 per product)"
                                 if frozen else None),
                           colour_branch_kernel_ms=color_avg),
             cpu_baseline=cpu,
@@ -629,7 +654,7 @@ def train_section(D, args, dev, cfg_name="ship_optimise", sparse=False, n_steps=
     out = dict(steps_per_s=1e3 / ms, ms_per_step=ms, ms_fwd=acc["forward"] / n_steps, ms_bwd=acc["backward"] / n_steps,
                ms_exchange=acc["exchange"] / n_steps, ms_adam=acc["adam"] / n_steps, ms_host_issue=host / n_steps * 1e3, mrays_per_s=3600 / ms / 1e3,
                hit_rays_per_step=hit / n_steps,
-               what="%s: N=%d, 3600 rays per step over %d rank(s), fwd (tcgen05) + bwd (tcgen05 GEMMs) + %s + 2x Adam over all N rows; "
+               what="%s: N=%d, 3600 rays per step over %d rank(s), fwd (wgmma) + bwd (wgmma GEMMs) + %s + 2x Adam over all N rows; "
                     "per-phase ms are rank 0's, ms_per_step the max over ranks"
                     % (cfg_name, cfg.N, D.world, "sparse touched-rows exchange of the point gradients + flat all-reduce of the MLP gradients" if sparse
                        else "one flat gradient all-reduce"))

@@ -1,5 +1,5 @@
 /*
- * pnb200 -- C ABI of the B200-native Point-NeRF per-ray hot path (libpnb200.so).
+ * pnb200 -- C ABI of the GPU-native (Hopper, sm_90a) Point-NeRF per-ray hot path (libpnb200.so).
  *
  * Plain C: pointers, sizes, a CUDA stream handle.  No torch types, no hidden allocations: every
  * device buffer (inputs, outputs, workspaces) is owned by the caller; *_bytes() functions report the
@@ -190,9 +190,9 @@ int pnb_aux_outputs(const pnb_query_t* q, const pnb_points_t* pts, const long lo
 int pnb_aux_conf_backward(const pnb_query_t* q, const long long* d_rows, int n_rows,
                           const float* d_grad_conf_coefficient, float* d_grad_conf, pnb_stream_t stream);
 
-/* ---- shading forward on the tensor cores (tcgen05 / TMEM, BF16x3 error-compensated split) ---- */
-/* Packs block1 / block3 / colour-branch weights of a pnb_mlp_t (fp32 W^T buffers) into tcgen05 operand images (hi/lo bf16, UMMA
- * shared-memory layout).  Call once per weight version.  d_out: >= pnb_mlp_pack_bytes() bytes. */
+/* ---- shading forward on the tensor cores (wgmma, BF16x3 error-compensated split) ---- */
+/* Packs block1 / block3 / colour-branch weights of a pnb_mlp_t (fp32 W^T buffers) into wgmma operand images (hi/lo bf16, one
+ * [N x 16] image pair per K step in the shared-memory operand layout).  Call once per weight version.  d_out: >= pnb_mlp_pack_bytes() bytes. */
 size_t pnb_mlp_pack_bytes(void);
 int pnb_mlp_pack(const pnb_mlp_t* mlp, void* d_out, size_t out_bytes, pnb_stream_t stream);
 /* Frozen point cloud (rendering): the 224 point-only inputs [f, PE3(f)] of block1.0
@@ -203,11 +203,10 @@ int pnb_point_pre(const pnb_points_t* pts, const pnb_mlp_t* mlp, float* d_pre, s
 enum {
     PNB_TC_PAIRS = 1,           /* row packing + per-pair MLPs + K-reduction -> h-bar, sigma */
     PNB_TC_COLOR = 2,           /* colour branch -> sigma_rgb (both = a forward) */
-    PNB_TC_FROZEN = 4,          /* pair kernel of a frozen cloud (k_shade_tc8): needs d_point_pre */
-    PNB_TC_DBG_NO_WEIGHTS = 64  /* timing experiment: no weight traffic (garbage results) */
-    /* bits 8..15: profiling flags of tools/tc_profile.py (1024: per-CTA cycles into d_err[64..], needs a 512-int d_err) */
+    PNB_TC_FROZEN = 4,          /* pair kernel of a frozen cloud (k_shade_wg<FROZEN>): needs d_point_pre */
+    PNB_TC_FEW_CTAS = 2048      /* test of the persistent tile loop: one CTA per 8 SMs instead of one per SM (same results) */
 };
-/* Same contract as pnb_shade_forward; the MLPs run as tcgen05.mma tiles.  mlp->w[5] must be zero padded to 288 rows.
+/* Same contract as pnb_shade_forward; the MLPs run as wgmma tiles.  mlp->w[5] must be zero padded to 288 rows.
  * ws >= pnb_shade_tc_bytes(max_valid_samples).  d_err: device int32[>= 64], 0 on success, 9 if the query produced more valid
  * samples than max_valid_samples (the extra samples are dropped: their sigma_rgb is zeroed, every other result is exact),
  * any other non-zero value = an internal pipeline time-out (a bounded 2-s mbarrier wait expired; results invalid). */
@@ -228,7 +227,7 @@ int pnb_shade_tc_tables(void* ws, size_t ws_bytes, int max_valid_samples, void**
  * points_conf [N] (any may be NULL) and of the 9 MLP layers in the layout of pnb_mlp_t (W^T [K_pad][N] and bias; the
  * caller zero-initialises all accumulators).  d_sigma_rgb_fwd: the forward's per-candidate (sigma, rgb) buffer.
  * n_valid / n_pairs: host copies of counters[PNB_QC_N_VALID] / [PNB_QC_N_PAIRS] (the pair-level buffers hold one row per valid pair).  ws >= pnb_backward_bytes.  The activations are recomputed and every layer
- * GEMM (recompute, dX, dW) runs on the tensor cores (tcgen05, BF16x3 split, fp32 accumulate; dW by a deterministic split-K);
+ * GEMM (recompute, dX, dW) runs on the tensor cores (wgmma, BF16x3 split, fp32 accumulate; dW by a deterministic split-K);
  * the recomputed pre-activations carry the BF16x3 error, so ~1e-6 of the LeakyReLU masks differ from an fp32 forward's (each changes
  * one pair's gradient by ~1/256; see the flags).  d_err: device int32,
  * set non-zero if a bounded pipeline wait of the tensor-core GEMMs expires (results invalid). */

@@ -17,6 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import ref_shim, query_oracle  # noqa: E402
+from oracle import golden  # noqa: E402
 from pointnerf_b200 import scene  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
@@ -79,7 +80,7 @@ def golden_case(name, cfg, pixels, alpha_bias, SR=24, extra_flags=()):
         fx["mlp." + k] = v.detach().numpy()
         fx["gradmlp." + k] = g["aggregator." + k].numpy()
     os.makedirs(OUT, exist_ok=True)
-    np.savez_compressed(os.path.join(OUT, name + ".npz"), **fx)
+    golden.save(OUT, name, fx)                                  # split into files < 1 MB (oracle/golden.py)
     print(name, "R'=%d" % fx["sample_pidx"].shape[0], "bgT mean %.3f" % fx["coarse_is_background"].mean(),
           {k: query_oracle.last_counters[k] for k in ("n_occ", "max_pts", "n_valid_samples", "n_valid_pairs")})
 

@@ -1,5 +1,5 @@
-"""Compile libpnb200.so (hand-written sm_100a CUDA + C ABI) in-tree with nvcc.  No torch involved.
-Also builds libpnb200_selftest.so (test-only tcgen05 self-tests / micro-benchmarks, csrc/selftest/)."""
+"""Compile libpnb200.so (hand-written sm_90a CUDA + C ABI) in-tree with nvcc.  No torch involved.
+Also builds libpnb200_selftest.so (test-only wgmma / GEMM-engine self-tests, csrc/selftest/)."""
 import glob
 import os
 import subprocess
@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libpnb200.so")
 LIB_SELFTEST = os.path.join(CSRC, "libpnb200_selftest.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--fmad=true", "-Xptxas", "-v"]
 
 

@@ -77,7 +77,7 @@ def validate(sd, opt=None):
 
 def load_into(net, path_or_dict, strict=True):
     """Loads a reference checkpoint into an existing NeuralPointsRayMarching (points are re-created as parameters, the
-    cached voxel grid is invalidated, the packed tcgen05 weight images are rebuilt on the next call)."""
+    cached voxel grid is invalidated, the packed wgmma weight images are rebuilt on the next call)."""
     sd = read_state_dict(path_or_dict)
     validate(sd, getattr(net, "opt", None))
     dev = net.neural_points.device

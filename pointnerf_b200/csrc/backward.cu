@@ -10,12 +10,12 @@
 //
 // Training batches are small (~2e4 valid samples), so the per-layer activations are recomputed into an HBM workspace and the
 // layer gradients are plain GEMMs: forward recompute  H = act(X W^T + b),  dX = (dZ W) * act'  and  dW += X^T dZ  all run on
-// the tensor cores (gemm_tc.cu: tcgen05 + TMEM, BF16x3 split, fp32 accumulate; the activation derivative is fused into the
+// the tensor cores (gemm_tc.cu: wgmma, BF16x3 split, fp32 accumulate; the activation derivative is fused into the
 // dX epilogue, dW is a deterministic split-K).
 // LeakyReLU masks: the recomputed pre-activations carry the BF16x3 error (~1e-5 relative), so ~1e-6 of the units (those whose
 // pre-activation is that close to zero) get the other mask than an fp32 forward would give them; each such unit changes ONE pair's
-// gradient by ~1/256 (measure-zero for the optimisation, visible in a max-abs comparison with fp32 autograd: tools/bwd_diag2.py lists
-// them).  A fix-up of the near-zero units cannot help - the perturbation comes from the inputs of the layer - and a three-part split
+// gradient by ~1/256 (measure-zero for the optimisation, visible in a max-abs comparison with fp32 autograd,
+// tests/test_gpu_backward.py bounds them).  A fix-up of the near-zero units cannot help - the perturbation comes from the inputs of the layer - and a three-part split
 // stops at ~1e-6 (tests/test_gpu_umma.py).  PNB_BWD_FP32_RECOMPUTE keeps the recompute on the fp32 CUDA-core tiles (fp32-faithful
 // masks, dX / dW still on the tensor cores); PNB_BWD_FP32_GEMM selects the hand-written fp32 CUDA-core tiles instead
 // (the parity reference of the tensor-core path; always used for the 128 -> 3 colour head).
@@ -120,7 +120,7 @@ static int gemm_nn(const GemmCtx& cx, const float* A, long lda, const float* Bt,
         GemmTc g{};
         g.A = A; g.a_rs = lda; g.a_ks = 1; g.B = Bt; g.b_rs = 1; g.b_ks = ldb; g.C = C; g.ldc = ldc; g.M = M; g.N = N; g.K = K;
         g.bias = bias; g.act = act; g.dact = nullptr; g.ldd = 0; g.dact_n = 0; g.err = cx.err; g.precise = cx.precise_all;
-        return gemm_tc(g, 1, cx.part, cx.part_bytes, 0, cx.st);     // (the split-K workspace doubles as the buffer of the weight images)
+        return gemm_tc(g, 1, cx.part, cx.part_bytes, 0, cx.st);
     }
     dim3 g((N + 63) / 64, (M + 127) / 128, 1);
     k_gemm<false><<<g, 256, 0, cx.st>>>(A, lda, 1, Bt, ldb, 1, C, ldc, M, N, K, K, bias, act);

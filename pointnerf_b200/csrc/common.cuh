@@ -1,4 +1,4 @@
-// Shared device/host helpers of libpnb200 (sm_100a only).
+// Shared device/host helpers of libpnb200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

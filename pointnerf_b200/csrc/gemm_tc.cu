@@ -1,21 +1,21 @@
-// Generic fp32-in / fp32-out GEMM on the 5th-generation tensor cores (tcgen05 + TMEM) with the BF16x3 error-compensated split
-// of shade_tc.cu -- the GEMM engine of the BACKWARD pass (backward.cu): forward recompute, dX = dZ . W and dW = X^T . dZ.
+// Generic fp32-in / fp32-out GEMM on the Hopper tensor cores (wgmma) with the BF16x3 error-compensated split of shade_tc.cu --
+// the GEMM engine of the BACKWARD pass (backward.cu): forward recompute, dX = dZ . W and dW = X^T . dZ.
 //
 //   C[M x N] = op( sum_k A(m,k) * B(n,k) + bias[n] )        A(m,k) = A[m*a_rs + k*a_ks],  B(n,k) = B[n*b_rs + k*b_ks]
 //
 // Either stride of an operand may be the unit one: operands whose reduction index is NOT contiguous in memory (W^T buffers,
 // the activations of dW = X^T dZ) are transposed on the way into shared memory, so the tensor cores only ever see the K-major
-// core-matrix layout that umma.cuh pins (tests/test_gpu_umma.py).  One CTA = one 128 x 128 output tile (UMMA M = 128, N = 128,
-// fp32 accumulator in 128 TMEM columns; two CTAs per SM), K blocks of 32 through a 2-stage shared-memory ring:
+// core-matrix layout of wgmma.cuh (tests/test_gpu_umma.py).  One CTA = one 128 x 128 output tile, two warpgroups of 64 rows each
+// (wgmma M = 64, N = 128, fp32 accumulators in registers), K blocks of 32 through a 2-stage shared-memory ring:
 //   warps 0-3  load the fp32 rows of A, split into bf16 hi / lo and store them in the operand layout; the next K block is already in
-//              registers while the current one is converted; afterwards the epilogue (thread = TMEM lane).  Lane mapping of a
-//              K block of 32 rows x 32 k per warp:
+//              registers while the current one is converted.  Lane mapping of a K block of 32 rows x 32 k per warp:
 //                * reduction index contiguous (ks == 1): load i of 8, lane l -> row 8(i/2) + (l/2)%8, floats 16(i%2) + 8(l/16) + 4(l%2) .. +3:
-//                  8 lines per LDG.128 (thread = row would touch 32 lines per request: 256 instead of 64 LSU wavefronts per block, which
-//                  is what bounded the first engine), and the 8-byte stores of a half warp fill one 128-byte run of the core-matrix layout;
+//                  8 lines per LDG.128 (thread = row would touch 32 lines per request), and the 8-byte stores of a half warp fill one
+//                  128-byte run of the core-matrix layout;
 //                * row index contiguous (transposing operands): thread = row, one coalesced LDG.32 per k
 //   warps 4-7  the same for the rows of B
-//   warp  8    issues 6 tcgen05.mma per K block (A_hi W_hi, A_lo W_hi, A_hi W_lo for the two K=16 steps), one commit per block
+//   all warps  then issue the wgmma of the block (A_hi B_hi, A_lo B_hi, A_hi B_lo for the two K = 16 steps; one group in flight)
+//              and finally run the epilogue from their accumulator fragments
 // PRECISE mode (forward recompute only): three bf16 parts per operand and the six products of total order <= 2 (a0b0, a1b0, a0b1,
 // a2b0, a1b1, a0b2): fp32-level pre-activations, so that the LeakyReLU masks of the backward are those of an fp32 forward (with the
 // BF16x3 recompute ~1e-5 of the units land on the other side of zero and each such flip changes a pair's gradient by ~1/256).
@@ -23,20 +23,18 @@
 // tile to a workspace; k_splitk_reduce adds the partials in split order (deterministic, no atomics).
 #include "common.cuh"
 #include "gemm_tc.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace pnb {
-using namespace umma;
+using namespace wg;
 
 namespace gtc {
-constexpr int TM = 128, TN = 128, LOG_NSTAGE = 1, NSTAGE = 1 << LOG_NSTAGE;    // 2 stages (64 KB): two CTAs per SM keep twice the loads in flight
+constexpr int TM = 128, TN = 128, NSTAGE = 2;
 constexpr int BLK = 128 * 64;             // [128 x 32] bf16 block
-constexpr int NTHR = 288;                 // warps 0-3: A loaders + epilogue, 4-7: B loaders, 8: issuer
+constexpr int NTHR = 256;                 // warps 0-3: A loaders, 4-7: B loaders; two wgmma warpgroups of 64 rows
 template <int NPART>
 struct Smem {
     unsigned char a[NPART][NSTAGE][BLK], b[NPART][NSTAGE][BLK];     // part 0 = hi, 1 = lo (mid), 2 = lo of the 3-part split
-    uint64_t bar_full[NSTAGE], bar_empty[NSTAGE], bar_acc;
-    uint32_t tmem_base;
 };
 // One K block (32 rows x 32 k of one loader warp) of an operand into registers / from registers into the NPART bf16 blocks of stage s.
 // COOP (ks == 1): v[4 i + c] = P(row 8(i/2) + (lane/2)%8, k0 + 16(i%2) + 8(lane/16) + 4(lane%2) + c); else v[e] = P(row lane, k0 + e).
@@ -100,360 +98,91 @@ __device__ __forceinline__ void store_blk(float* v, unsigned char (*blk)[NSTAGE]
         }
     }
 }
-// the loader loop of one warp: K blocks kbeg .. kend of its 32 rows through the ring
-template <int NPART, bool COOP, class SmemT>
-__device__ __forceinline__ bool load_rows(SmemT& sm, unsigned char (*blk)[NSTAGE][BLK], const float* __restrict__ P, long rs, long ks, long R0, int w, int lane,
-                                          long nrows, int kbeg, int kend, int nkb, int* err) {
-    float cur[32], nxt[32];
-    fetch_blk<COOP>(P, rs, ks, R0, w, lane, nrows, kbeg, kend, cur);
-    for (int kb = 0; kb < nkb; ++kb) {
-        const uint32_t s = (uint32_t)kb & (NSTAGE - 1), ph = ((uint32_t)kb >> LOG_NSTAGE) & 1u;
-        if (kb + 1 < nkb) fetch_blk<COOP>(P, rs, ks, R0, w, lane, nrows, kbeg + 32 * (kb + 1), kend, nxt);
-        if (!mbar_wait(&sm.bar_empty[s], ph ^ 1u, err, 72)) return false;
-        store_blk<NPART, COOP>(cur, blk, (int)s, w, lane);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sm.bar_full[s]);   // (32 same-address arrives would serialise in the shared-memory atomic unit)
-#pragma unroll
-        for (int e = 0; e < 32; ++e) cur[e] = nxt[e];
-    }
-    return true;
-}
 }  // namespace gtc
 
 template <bool PRECISE>
-__global__ void __launch_bounds__(gtc::NTHR, 2) k_gemm_tc(GemmTc g) {
+__global__ void __launch_bounds__(gtc::NTHR, 1) k_gemm_tc(GemmTc g) {
     using namespace gtc;
     constexpr int NPART = PRECISE ? 3 : 2;
     using SmemT = Smem<NPART>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemT& sm = *reinterpret_cast<SmemT*>(smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u));
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2;
     const int m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
     const int kbeg = blockIdx.z * g.kchunk, kend = min(g.K, kbeg + g.kchunk);
     const int nkb = (kend - kbeg + 31) >> 5;
 
-    if (tid == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&sm.bar_full[s], 8); mbar_init(&sm.bar_empty[s], 1); }   // one arrive per loader warp
-        mbar_init(&sm.bar_acc, 1);
-        mbar_fence_init();
-    }
-    if (warp == 8) tmem_alloc<128>(&sm.tmem_base);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tacc = sm.tmem_base;
+    // loaders: warps 0-3 own the A rows, warps 4-7 the B rows (32 rows per warp); the NEXT K block is fetched into registers before
+    // the current one is converted and stored, so a full K block of loads is in flight per thread
+    const bool isB = warp >= 4;
+    const float* P = isB ? g.B : g.A;
+    const long rs = isB ? g.b_rs : g.a_rs, ks = isB ? g.b_ks : g.a_ks;
+    const long R0 = isB ? n0 : m0, nrows = isB ? g.N : g.M;
+    const int w32 = (tid & 127) & ~31;
+    const bool coop = ks == 1;
+    unsigned char (*blk)[NSTAGE][BLK] = isB ? sm.b : sm.a;
+    float cur[32], nxt[32];
+    if (coop) fetch_blk<true>(P, rs, ks, R0, w32, lane, nrows, kbeg, kend, cur);
+    else fetch_blk<false>(P, rs, ks, R0, w32, lane, nrows, kbeg, kend, cur);
 
-    if (warp == 8) {
-        const uint32_t idesc = make_idesc_bf16(128, 128);
-        const uint32_t hiw = desc_hi<LAYOUT_NONE>();
-        uint32_t a0[NPART], b0[NPART];
+    float acc[64];
 #pragma unroll
-        for (int i = 0; i < NPART; ++i) { a0[i] = desc_lo<LAYOUT_NONE>(smem_u32(sm.a[i][0])); b0[i] = desc_lo<LAYOUT_NONE>(smem_u32(sm.b[i][0])); }
-        constexpr uint32_t KADV = kstep_adv16<LAYOUT_NONE>(), SADV = BLK >> 4;
-        bool ok = true;
-        for (int kb = 0; kb < nkb && ok; ++kb) {
-            const uint32_t s = (uint32_t)kb & (NSTAGE - 1), ph = ((uint32_t)kb >> LOG_NSTAGE) & 1u;
-            if (!mbar_wait(&sm.bar_full[s], ph, g.err, 71)) { ok = false; break; }
-            tc_fence_after();
-            bool first = kb == 0;
-#pragma unroll
-            for (int i = 0; i < NPART; ++i)
-#pragma unroll
-                for (int j = 0; j < NPART; ++j) {
-                    if (i + j >= NPART) continue;          // products of total order < NPART: 3 (BF16x3) or 6 (3-part split)
-                    const uint32_t ad = a0[i] + s * SADV, bd = b0[j] + s * SADV;
-                    mma_ss2_w(tacc, ad, hiw, bd, hiw, idesc, first ? 0u : 1u);
-                    mma_ss2_w(tacc, ad + KADV, hiw, bd + KADV, hiw, idesc, 1u);
-                    first = false;
-                }
-            mma_commit_w(&sm.bar_empty[s]);
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    const uint32_t a0 = smem_u32(sm.a[0][0]) + (uint32_t)wgi * 4096u, b0 = smem_u32(sm.b[0][0]);
+    constexpr uint32_t PART = NSTAGE * BLK;                  // byte distance between the parts of an operand
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb & (NSTAGE - 1);
+        if (kb + 1 < nkb) {
+            if (coop) fetch_blk<true>(P, rs, ks, R0, w32, lane, nrows, kbeg + 32 * (kb + 1), kend, nxt);
+            else fetch_blk<false>(P, rs, ks, R0, w32, lane, nrows, kbeg + 32 * (kb + 1), kend, nxt);
         }
-        mma_commit_w(&sm.bar_acc);
-    } else {
-        // loaders: warps 0-3 own the A rows (thread = tile row), warps 4-7 the B rows; the NEXT K block is fetched into registers
-        // before the current one is converted and stored, so a full K block of loads is in flight per thread
-        const bool isB = warp >= 4;
-        const int t = tid & 127, lane = tid & 31;
-        const float* P = isB ? g.B : g.A;
-        const long rs = isB ? g.b_rs : g.a_rs, ks = isB ? g.b_ks : g.a_ks;
-        const long R0 = isB ? n0 : m0, nrows = isB ? g.N : g.M;
-        const long r = R0 + t;
-        const bool row_ok = r < nrows;
-        unsigned char (*blk)[NSTAGE][BLK] = isB ? sm.b : sm.a;
-        const bool ok = ks == 1 ? load_rows<NPART, true>(sm, blk, P, rs, ks, R0, t & ~31, lane, nrows, kbeg, kend, nkb, g.err)
-                                : load_rows<NPART, false>(sm, blk, P, rs, ks, R0, t & ~31, lane, nrows, kbeg, kend, nkb, g.err);
-        if (!isB && ok && mbar_wait(&sm.bar_acc, 0u, g.err, 73)) {
-            tc_fence_after();
-            const long ra = r;
-            const bool a_ok = row_ok;
-            const uint32_t tl = tacc + ((uint32_t)(warp * 32) << 16);
-            float* crow = g.part ? g.part + ((size_t)blockIdx.z * g.M + (size_t)ra) * g.N : g.C + ra * g.ldc;
-#pragma unroll 1
-            for (int c = 0; c < TN / 16; ++c) {
-                const int n = n0 + 16 * c;
-                uint32_t v[16];
-                tmem_ld16(tl + (uint32_t)(16 * c), v);      // all lanes of the warp (sync.aligned), also those of rows >= M
-                tmem_ld_wait();
-                if (!a_ok || n >= g.N) continue;
-                float y[16];
+        named_bar_sync(1, NTHR);                     // both warpgroups have retired the wgmma group of block kb - 2 (stage s)
+        if (coop) store_blk<NPART, true>(cur, blk, s, w32, lane);
+        else store_blk<NPART, false>(cur, blk, s, w32, lane);
+        fence_proxy_async();
+        named_bar_sync(1, NTHR);
+        wg::fence();
 #pragma unroll
-                for (int e = 0; e < 16; ++e) y[e] = __uint_as_float(v[e]);
-                if (!g.part) {
-                    if (g.bias) {
+        for (int i = 0; i < NPART; ++i)
 #pragma unroll
-                        for (int e = 0; e < 16; ++e) y[e] += __ldg(g.bias + n + e);
-                    }
-                    if (g.act) {
-#pragma unroll
-                        for (int e = 0; e < 16; ++e) y[e] = fmaxf(y[e], 0.01f * y[e]);
-                    }
-                    if (g.dact && n < g.dact_n) {            // backward of the LeakyReLU below: * (Y > 0 ? 1 : 0.01)
-                        const float4* yp = reinterpret_cast<const float4*>(g.dact + ra * g.ldd + n);
-#pragma unroll
-                        for (int e4 = 0; e4 < 4; ++e4) {
-                            const float4 yy = __ldg(yp + e4);
-                            y[4 * e4] *= yy.x > 0.f ? 1.0f : 0.01f; y[4 * e4 + 1] *= yy.y > 0.f ? 1.0f : 0.01f;
-                            y[4 * e4 + 2] *= yy.z > 0.f ? 1.0f : 0.01f; y[4 * e4 + 3] *= yy.w > 0.f ? 1.0f : 0.01f;
-                        }
-                    }
-                }
-                float4* dst = reinterpret_cast<float4*>(crow + n);
-#pragma unroll
-                for (int e4 = 0; e4 < 4; ++e4) dst[e4] = make_float4(y[4 * e4], y[4 * e4 + 1], y[4 * e4 + 2], y[4 * e4 + 3]);
+            for (int j = 0; j < NPART; ++j) {
+                if (i + j >= NPART) continue;          // products of total order < NPART: 3 (BF16x3) or 6 (3-part split)
+                const uint32_t ad = a0 + (uint32_t)i * PART + (uint32_t)s * BLK, bd = b0 + (uint32_t)j * PART + (uint32_t)s * BLK;
+                mma_n128(acc, desc_none(ad), desc_none(bd), (kb > 0 || i + j > 0) ? 1u : 0u);
+                mma_n128(acc, desc_none(ad + 256u), desc_none(bd + 256u), 1u);
             }
-        }
+        wg::commit();
+        wg::wait<1>();
+#pragma unroll
+        for (int e = 0; e < 32; ++e) cur[e] = nxt[e];
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 8) tmem_dealloc<128>(sm.tmem_base);
-}
-
-// =====================================================================================================================
-// k_gemm_tcw: the same product for the case "B is small and shared by all M tiles" (every forward-recompute and dX GEMM of the
-// backward: B = a weight matrix, <= 288 x 288).  What bounded k_gemm_tc there was operand delivery, not the tensor pipe: every 128 x 128
-// tile converted its own 128 x K slab of the WEIGHTS from fp32, and A was read once per 128 output columns.  Here
-//   * B is converted ONCE per GEMM into bf16 hi / lo operand images (k_pack_bimg: [K block][hi | lo][Npad x 32], core-matrix layout) and
-//     streamed by the TMA engine (cp.async.bulk, one elected thread, no conversion work in the tile);
-//   * one CTA owns a 128 x (<= 256) tile: full rows of a 256-wide layer, so A is read and converted once (MMA N = 256);
-//   * all 8 loader warps work on A (16 rows each), afterwards all 8 run the epilogue (TMEM lane quarter = warp % 4, column half = warp / 4).
-// Two CTAs per SM (96 KB of shared memory, 256 TMEM columns each).
-namespace gtw {
-constexpr int TM = 128, TNMAX = 256, NSTAGE = 2;
-constexpr int ABLK = 128 * 64;              // [128 x 32] bf16 block of A
-constexpr int BIMG = TNMAX * 64;            // [256 x 32] bf16 image of B (one part)
-constexpr int NTHR = 320;                   // warps 0-7: A loaders + epilogue, 8: MMA issuer, 9: B loader
-struct Smem {
-    unsigned char a[2][NSTAGE][ABLK];       // part 0 = hi, 1 = lo
-    unsigned char b[NSTAGE][2][BIMG];
-    uint64_t bar_a[NSTAGE], bar_b[NSTAGE], bar_empty[NSTAGE], bar_acc;
-    uint32_t tmem_base;
-};
-}  // namespace gtw
-
-// B(n,k) = B[n*b_rs + k*b_ks], n < N, k < K  ->  img[kb][part][Npad x 32] (zero padded), one thread per (n, 8 k)
-__global__ void __launch_bounds__(256) k_pack_bimg(const float* __restrict__ B, long b_rs, long b_ks, int N, int K, int Npad, int nkb, unsigned char* __restrict__ img) {
-    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (long)nkb * 4 * Npad) return;
-    const int n = (int)(i % Npad), oc = (int)((i / Npad) & 3), kb = (int)(i / (4L * Npad));
-    float v[8];
+    wg::wait<0>();
+    pin<64>(acc);
+    if (nkb == 0) return;
+    // ---------------- epilogue from the accumulator fragments: rows r0, r0 + 8, columns n0 + 8j + cq, +1
+    const long r0 = (long)m0 + 64 * wgi + 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-        const int k = kb * 32 + oc * 8 + e;
-        v[e] = (n < N && k < K) ? __ldg(B + n * b_rs + (long)k * b_ks) : 0.f;
-    }
-    const uint32_t off = umma::tile_offset_bytes<umma::LAYOUT_NONE>(n, 8 * oc);
+    for (int h = 0; h < 2; ++h) {
+        const long ra = r0 + 8 * h;
+        if (ra >= g.M) continue;
+        float* crow = g.part ? g.part + ((size_t)blockIdx.z * g.M + (size_t)ra) * g.N : g.C + ra * g.ldc;
 #pragma unroll
-    for (int part = 0; part < 2; ++part) {
-        uint32_t w[4];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * c], v[2 * c + 1]);
-            v[2 * c] -= __low2float(h); v[2 * c + 1] -= __high2float(h);
-            w[c] = *reinterpret_cast<const uint32_t*>(&h);
-        }
-        *reinterpret_cast<uint4*>(img + ((size_t)kb * 2 + part) * (size_t)Npad * 64 + off) = make_uint4(w[0], w[1], w[2], w[3]);
-    }
-}
-
-__global__ void __launch_bounds__(gtw::NTHR, 2) k_gemm_tcw(GemmTc g, const unsigned char* __restrict__ bimg, int Npad) {
-    using namespace gtw;
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    Smem& sm = *reinterpret_cast<Smem*>(smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u));
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m0 = blockIdx.y * TM, n0 = blockIdx.x * TNMAX;
-    const int tn = min(TNMAX, Npad - n0);                  // multiple of 16
-    const int nkb = (g.K + 31) >> 5;
-
-    if (tid == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&sm.bar_a[s], 8); mbar_init(&sm.bar_b[s], 1); mbar_init(&sm.bar_empty[s], 1); }
-        mbar_init(&sm.bar_acc, 1);
-        mbar_fence_init();
-    }
-    if (warp == 8) tmem_alloc<256>(&sm.tmem_base);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tacc = sm.tmem_base;
-
-    if (warp == 9) {
-        // ---------------- B: two bulk copies (hi, lo rows n0 .. n0+tn of the K block's images) per stage
-        if (lane == 0) {
-            for (int kb = 0; kb < nkb; ++kb) {
-                const uint32_t s = (uint32_t)kb & 1u, ph = ((uint32_t)kb >> 1) & 1u;
-                if (!mbar_wait(&sm.bar_empty[s], ph ^ 1u, g.err, 75)) break;
-                const uint32_t bytes = (uint32_t)tn * 64u;
-                mbar_arrive_expect_tx(&sm.bar_b[s], 2u * bytes);
-                const unsigned char* src = bimg + ((size_t)kb * 2) * (size_t)Npad * 64 + (size_t)n0 * 64;
-                bulk_g2s(sm.b[s][0], src, bytes, &sm.bar_b[s]);
-                bulk_g2s(sm.b[s][1], src + (size_t)Npad * 64, bytes, &sm.bar_b[s]);
-            }
-        }
-    } else if (warp == 8) {
-        // ---------------- MMA issuer: A_hi B_hi + A_lo B_hi + A_hi B_lo for the two K = 16 steps of a block, one commit per block
-        const uint32_t idesc = make_idesc_bf16(128, tn);
-        const uint32_t hiw = desc_hi<LAYOUT_NONE>();
-        const uint32_t ah0 = desc_lo<LAYOUT_NONE>(smem_u32(sm.a[0][0])), al0 = desc_lo<LAYOUT_NONE>(smem_u32(sm.a[1][0]));
-        const uint32_t bh0 = desc_lo<LAYOUT_NONE>(smem_u32(sm.b[0][0])), bl0 = desc_lo<LAYOUT_NONE>(smem_u32(sm.b[0][1]));
-        constexpr uint32_t KADV = kstep_adv16<LAYOUT_NONE>(), ASADV = ABLK >> 4, BSADV = (2 * BIMG) >> 4;
-        for (int kb = 0; kb < nkb; ++kb) {
-            const uint32_t s = (uint32_t)kb & 1u, ph = ((uint32_t)kb >> 1) & 1u;
-            if (!mbar_wait(&sm.bar_b[s], ph, g.err, 76)) break;
-            if (!mbar_wait(&sm.bar_a[s], ph, g.err, 71)) break;
-            tc_fence_after();
-            const uint32_t ah = ah0 + s * ASADV, al = al0 + s * ASADV, bh = bh0 + s * BSADV, bl = bl0 + s * BSADV;
-            mma_ss2_w(tacc, ah, hiw, bh, hiw, idesc, kb ? 1u : 0u);
-            mma_ss2_w(tacc, al, hiw, bh, hiw, idesc, 1u);
-            mma_ss2_w(tacc, ah + KADV, hiw, bh + KADV, hiw, idesc, 1u);
-            mma_ss2_w(tacc, al + KADV, hiw, bh + KADV, hiw, idesc, 1u);
-            mma_ss2_w(tacc, ah, hiw, bl, hiw, idesc, 1u);
-            mma_ss2_w(tacc, ah + KADV, hiw, bl + KADV, hiw, idesc, 1u);
-            mma_commit_w(&sm.bar_empty[s]);
-        }
-        mma_commit_w(&sm.bar_acc);
-    } else {
-        // ---------------- A: warp w owns tile rows 16w .. 16w+15; two K blocks of loads in flight per thread
-        // reduction index contiguous: load i of 4, lane l -> row 16w + 8(i/2) + (l/2)%8, floats 16(i%2) + 8(l/16) + 4(l%2) .. +3
-        // row index contiguous (transposing): thread -> row 16w + l%16, k = 16(l/16) + e: 16 LDG.32, each 64 contiguous bytes per half warp
-        const bool coop = g.a_ks == 1;
-        const int w16 = warp * 16;
-        auto fetch = [&](int k0, float* v) {
-            if (coop) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const long r = (long)m0 + w16 + 8 * (i >> 1) + ((lane >> 1) & 7);
-                    const int k = k0 + 16 * (i & 1) + 8 * (lane >> 4) + 4 * (lane & 1);
-                    if (r < g.M && k + 4 <= g.K) {
-                        const float4 x = __ldg(reinterpret_cast<const float4*>(g.A + r * g.a_rs + k));
-                        v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
-                    } else {
-#pragma unroll
-                        for (int c = 0; c < 4; ++c) v[4 * i + c] = (r < g.M && k + c < g.K) ? __ldg(g.A + r * g.a_rs + k + c) : 0.f;
-                    }
-                }
-            } else {
-                const long r = (long)m0 + w16 + (lane & 15);
-                const int kq = k0 + 16 * (lane >> 4);
-#pragma unroll
-                for (int e = 0; e < 16; ++e) v[e] = (r < g.M && kq + e < g.K) ? __ldg(g.A + r * g.a_rs + (long)(kq + e) * g.a_ks) : 0.f;
-            }
-        };
-        auto store = [&](float* v, int s) {
-            if (coop) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int t = w16 + 8 * (i >> 1) + ((lane >> 1) & 7);
-                    const uint32_t off = tile_offset_bytes<LAYOUT_NONE>(t, 16 * (i & 1) + 8 * (lane >> 4)) + 8u * (uint32_t)(lane & 1);
-#pragma unroll
-                    for (int part = 0; part < 2; ++part) {
-                        uint32_t ww[2];
-#pragma unroll
-                        for (int c = 0; c < 2; ++c) {
-                            const __nv_bfloat162 h = __floats2bfloat162_rn(v[4 * i + 2 * c], v[4 * i + 2 * c + 1]);
-                            v[4 * i + 2 * c] -= __low2float(h); v[4 * i + 2 * c + 1] -= __high2float(h);
-                            ww[c] = *reinterpret_cast<const uint32_t*>(&h);
-                        }
-                        *reinterpret_cast<uint2*>(sm.a[part][s] + off) = make_uint2(ww[0], ww[1]);
-                    }
-                }
-            } else {
-                const int t = w16 + (lane & 15);
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    const uint32_t off = tile_offset_bytes<LAYOUT_NONE>(t, 16 * (lane >> 4) + 8 * c);
-#pragma unroll
-                    for (int part = 0; part < 2; ++part) {
-                        uint32_t ww[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const __nv_bfloat162 h = __floats2bfloat162_rn(v[8 * c + 2 * i], v[8 * c + 2 * i + 1]);
-                            v[8 * c + 2 * i] -= __low2float(h); v[8 * c + 2 * i + 1] -= __high2float(h);
-                            ww[i] = *reinterpret_cast<const uint32_t*>(&h);
-                        }
-                        *reinterpret_cast<uint4*>(sm.a[part][s] + off) = make_uint4(ww[0], ww[1], ww[2], ww[3]);
-                    }
-                }
-            }
-        };
-        float v0[16], v1[16], v2[16];
-        fetch(0, v0);
-        if (nkb > 1) fetch(32, v1);
-        bool ok = true;
-        for (int kb = 0; kb < nkb; ++kb) {
-            const uint32_t s = (uint32_t)kb & 1u, ph = ((uint32_t)kb >> 1) & 1u;
-            if (kb + 2 < nkb) fetch(32 * (kb + 2), v2);
-            if (!mbar_wait(&sm.bar_empty[s], ph ^ 1u, g.err, 72)) { ok = false; break; }
-            store(v0, (int)s);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.bar_a[s]);
-#pragma unroll
-            for (int e = 0; e < 16; ++e) { v0[e] = v1[e]; v1[e] = v2[e]; }
-        }
-        // ---------------- epilogue: TMEM lane quarter = warp % 4, 16-column chunks c = warp/4, warp/4 + 2, ...
-        if (ok && mbar_wait(&sm.bar_acc, 0u, g.err, 73)) {
-            tc_fence_after();
-            const int q = warp & 3;
-            const long ra = (long)m0 + q * 32 + lane;
-            const bool a_ok = ra < g.M;
-            const uint32_t tl = tacc + ((uint32_t)(q * 32) << 16);
-            float* crow = g.C + ra * g.ldc;
-#pragma unroll 1
-            for (int c = warp >> 2; c < tn / 16; c += 2) {
-                const int n = n0 + 16 * c;
-                uint32_t v[16];
-                tmem_ld16(tl + (uint32_t)(16 * c), v);      // all lanes of the warp (sync.aligned), also those of rows >= M
-                tmem_ld_wait();
-                if (!a_ok || n >= g.N) continue;
-                float y[16];
-#pragma unroll
-                for (int e = 0; e < 16; ++e) y[e] = __uint_as_float(v[e]);
-                if (g.bias) {
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) y[e] += __ldg(g.bias + n + e);
-                }
-                if (g.act) {
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) y[e] = fmaxf(y[e], 0.01f * y[e]);
-                }
+        for (int j = 0; j < 16; ++j) {
+            const int n = n0 + 8 * j + cq;
+            if (n >= g.N) continue;
+            float y0 = acc[4 * j + 2 * h], y1 = acc[4 * j + 2 * h + 1];
+            if (!g.part) {
+                if (g.bias) { y0 += __ldg(g.bias + n); y1 += __ldg(g.bias + n + 1); }
+                if (g.act) { y0 = fmaxf(y0, 0.01f * y0); y1 = fmaxf(y1, 0.01f * y1); }
                 if (g.dact && n < g.dact_n) {            // backward of the LeakyReLU below: * (Y > 0 ? 1 : 0.01)
-                    const float4* yp = reinterpret_cast<const float4*>(g.dact + ra * g.ldd + n);
-#pragma unroll
-                    for (int e4 = 0; e4 < 4; ++e4) {
-                        const float4 yy = __ldg(yp + e4);
-                        y[4 * e4] *= yy.x > 0.f ? 1.0f : 0.01f; y[4 * e4 + 1] *= yy.y > 0.f ? 1.0f : 0.01f;
-                        y[4 * e4 + 2] *= yy.z > 0.f ? 1.0f : 0.01f; y[4 * e4 + 3] *= yy.w > 0.f ? 1.0f : 0.01f;
-                    }
+                    const float2 yy = __ldg(reinterpret_cast<const float2*>(g.dact + ra * g.ldd + n));
+                    y0 *= yy.x > 0.f ? 1.0f : 0.01f; y1 *= yy.y > 0.f ? 1.0f : 0.01f;
                 }
-                float4* dst = reinterpret_cast<float4*>(crow + n);
-#pragma unroll
-                for (int e4 = 0; e4 < 4; ++e4) dst[e4] = make_float4(y[4 * e4], y[4 * e4 + 1], y[4 * e4 + 2], y[4 * e4 + 3]);
             }
+            *reinterpret_cast<float2*>(crow + n) = make_float2(y0, y1);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 8) tmem_dealloc<256>(sm.tmem_base);
 }
 
 // C[m][n] (+)= sum_z part[z][m][n], z ascending
@@ -473,6 +202,7 @@ int gemm_tc(const GemmTc& g0, int splits, float* part_ws, size_t part_bytes, int
     PNB_REQUIRE((g.a_rs == 1) != (g.a_ks == 1) || g.K == 1 || g.M == 1, PNB_ERR_INVALID, "gemm_tc: one stride of A must be 1");
     PNB_REQUIRE(g.a_ks != 1 || g.a_rs % 4 == 0, PNB_ERR_INVALID, "gemm_tc: leading dimension of A must be a multiple of 4");
     PNB_REQUIRE(g.b_ks != 1 || g.b_rs % 4 == 0, PNB_ERR_INVALID, "gemm_tc: leading dimension of B must be a multiple of 4");
+    PNB_REQUIRE(g.dact == nullptr || g.ldd % 2 == 0, PNB_ERR_INVALID, "gemm_tc: leading dimension of dact must be even");
     static int configured[64] = {0};
     int dev = 0;
     PNB_CHECK_CUDA(cudaGetDevice(&dev));
@@ -483,25 +213,6 @@ int gemm_tc(const GemmTc& g0, int splits, float* part_ws, size_t part_bytes, int
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_gemm_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(gtc::Smem<2>) + 128)));
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_gemm_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(gtc::Smem<3>) + 128)));
         configured[dev] = 1;
-    }
-    // weights-as-images path: B small (the whole GEMM shares it), no split-K, BF16x3; the caller's workspace holds the images
-    const int Npad = (g.N + 15) / 16 * 16, nkb_all = (g.K + 31) / 32;
-    const size_t img_bytes = (size_t)nkb_all * 2 * Npad * 64;
-    if (splits <= 1 && !precise && !accumulate && part_ws && part_bytes >= img_bytes && g.N <= 1024 && g.K <= 1024 && (g.a_ks != 1 || g.a_rs % 4 == 0) &&
-        (g.dact == nullptr || g.ldd % 4 == 0)) {
-        static int configured_w[64] = {0};
-        if (dev >= 0 && dev < 64 && !configured_w[dev]) {
-            PNB_CHECK_CUDA(cudaFuncSetAttribute(k_gemm_tcw, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(gtw::Smem) + 128)));
-            configured_w[dev] = 1;
-        }
-        g.kchunk = g.K; g.part = nullptr;
-        unsigned char* img = reinterpret_cast<unsigned char*>(part_ws);
-        const long nthr = (long)nkb_all * 4 * Npad;
-        k_pack_bimg<<<(int)((nthr + 255) / 256), 256, 0, st>>>(g.B, g.b_rs, g.b_ks, g.N, g.K, Npad, nkb_all, img);
-        dim3 grid((Npad + gtw::TNMAX - 1) / gtw::TNMAX, (g.M + gtw::TM - 1) / gtw::TM, 1);
-        k_gemm_tcw<<<grid, gtw::NTHR, sizeof(gtw::Smem) + 128, st>>>(g, img, Npad);
-        PNB_CHECK_CUDA(cudaGetLastError());
-        return PNB_OK;
     }
     if (splits <= 1) {
         g.kchunk = g.K; g.part = nullptr;

@@ -1,4 +1,4 @@
-// tcgen05 BF16x3 GEMM of the backward pass (gemm_tc.cu).
+// wgmma BF16x3 GEMM of the backward pass (gemm_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

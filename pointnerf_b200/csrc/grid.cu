@@ -4,7 +4,7 @@
 //   claim_occ      /root/reference/models/neural_points/cuda/query_worldcoords.cu:18-78
 //   map_coor2occ   :80-115
 //   fill_occ2pnts  :117-162
-// and the three dense int32 grids of :314-319.  Layout here (B200: everything the ray march touches is a
+// and the three dense int32 grids of :314-319.  Layout here (everything the ray march touches is a
 // 1-bit-per-voxel mask that stays in L2/L1; points of one voxel are contiguous 16-byte records):
 //   occ_bits   dilated occupancy, the reference's coor_occ
 //   pt_bits    voxels holding points; slot(cell) = word_rank[cell>>5] + popc(pt_bits[cell>>5] & below)

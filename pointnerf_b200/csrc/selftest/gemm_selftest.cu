@@ -1,4 +1,4 @@
-// TEST-ONLY (libpnb200_selftest.so): C entry point over the tcgen05 GEMM engine of the backward pass (../gemm_tc.cu, compiled
+// TEST-ONLY (libpnb200_selftest.so): C entry point over the wgmma GEMM engine of the backward pass (../gemm_tc.cu, compiled
 // into this library a second time) so that tests/test_gpu_umma.py can compare every operand form with a torch matmul.
 #include "../gemm_tc.cu"
 #include "pnb200_selftest.h"

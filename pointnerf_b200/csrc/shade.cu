@@ -1,5 +1,5 @@
 // Fused gather + distance weights + positional encoding + MLP chain + K-reduction + colour branch (forward),
-// fp32 CUDA-core version ("v1": the exact-fp32 path; the tcgen05 BF16x3 path lives in shade_tc.cu).
+// fp32 CUDA-core version ("v1": the exact-fp32 path; the wgmma BF16x3 path lives in shade_tc.cu).
 //
 // Replaces, per valid sample tile, what the reference does with ~40 eager torch kernels and HBM round trips:
 //   gather                     /root/reference/models/neural_points/neural_points.py:706-717

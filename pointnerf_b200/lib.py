@@ -61,9 +61,9 @@ SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes",
            "pnb_shade_tc_tables", "pnb_backward_bytes", "pnb_shade_backward", "pnb_aux_outputs", "pnb_aux_conf_backward"]
 # test-only library (csrc/selftest/pnb200_selftest.h)
 SELFTEST_LIB_PATH = os.path.join(_HERE, "csrc", "libpnb200_selftest.so")
-SELFTEST_SYMBOLS = ["pnb_selftest_last_error", "pnb_umma_selftest", "pnb_umma_bench", "pnb_umma_selftest2", "pnb_gemm_tc_test"]
+SELFTEST_SYMBOLS = ["pnb_selftest_last_error", "pnb_umma_selftest", "pnb_umma_selftest2", "pnb_gemm_tc_test"]
 # flags of pnb_shade_forward_tc
-TC_PAIRS, TC_COLOR, TC_FROZEN, TC_DBG_NO_WEIGHTS = 1, 2, 4, 64
+TC_PAIRS, TC_COLOR, TC_FROZEN = 1, 2, 4
 BWD_FP32_GEMM, BWD_FP32_RECOMPUTE = 1, 4   # flags of pnb_shade_backward
 
 _lib = None
@@ -76,7 +76,7 @@ def load():
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise PnbError("libpnb200.so not found at %s -- run `python -m pointnerf_b200.build` (nvcc, sm_100a). "
+        raise PnbError("libpnb200.so not found at %s -- run `python -m pointnerf_b200.build` (nvcc, sm_90a). "
                        "There is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     lib.pnb_version.restype = C.c_int
@@ -143,7 +143,7 @@ def load():
 
 
 def load_selftest():
-    """Test-only library with the tcgen05 self-tests / micro-benchmarks (not part of the product ABI)."""
+    """Test-only library with the wgmma and GEMM-engine self-tests (not part of the product ABI)."""
     global _selftest
     if _selftest is not None:
         return _selftest
@@ -151,11 +151,8 @@ def load_selftest():
         raise PnbError("libpnb200_selftest.so not found at %s -- run `python -m pointnerf_b200.build`" % SELFTEST_LIB_PATH)
     lib = C.CDLL(SELFTEST_LIB_PATH)
     lib.pnb_selftest_last_error.restype = C.c_char_p
-    lib.pnb_umma_bench.restype = C.c_int
-    lib.pnb_umma_bench.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.pnb_umma_selftest2.restype = C.c_int
-    lib.pnb_umma_selftest2.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
-                                       C.c_void_p, C.c_void_p]
+    lib.pnb_umma_selftest2.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.pnb_umma_selftest.restype = C.c_int
     lib.pnb_umma_selftest.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.pnb_gemm_tc_test.restype = C.c_int

@@ -108,7 +108,7 @@ class MlpPack:
         self.wt = None
         self.bias = None
         self.desc = None
-        self.packed = None   # tcgen05 operand images of block1/block3 (hi/lo bf16)
+        self.packed = None   # wgmma operand images of block1/block3 and the colour branch (hi/lo bf16)
         self.key_l1 = None   # version key of block1.0 (weight, bias): what the hoisted per-point table depends on
 
     def get(self, agg):
@@ -237,7 +237,7 @@ class NeuralPoints(nn.Module):
 
 class _RenderFn(torch.autograd.Function):
     """Differentiable face of the fused path: ray_color[R,3] = f(points_embeding, points_color, points_dir,
-    points_conf, 18 MLP tensors).  Backward = pnb_shade_backward (activations recomputed, layer GEMMs on tcgen05 / BF16x3)."""
+    points_conf, 18 MLP tensors).  Backward = pnb_shade_backward (activations recomputed, layer GEMMs on wgmma / BF16x3)."""
 
     @staticmethod
     def forward(ctx, mod, run_args, emb, color, pdir, conf, *mlp_params):
@@ -355,7 +355,7 @@ def _init_state(mod):
     mod._status_pending = []     # (event, pinned [err, query counters], R) of render_full() calls not yet checked
     mod._status_free = []
     mod._max_valid = 0
-    # "bf16x3": per-pair MLPs on tcgen05 tensor cores with the error-compensated split (default);
+    # "bf16x3": per-pair MLPs on wgmma tensor cores with the error-compensated split (default);
     # "fp32": the exact-fp32 CUDA-core kernel.
     mod.precision = getattr(opt, "pnb_precision", "bf16x3")
     if mod.precision not in ("bf16x3", "fp32"):
@@ -425,14 +425,14 @@ class NeuralPointsRayMarching(nn.Module):
             self._status_free.append(host)
             if bwd_err != 0:
                 self._bwd_err.zero_()
-                raise _lib.PnbError("pnb200: tcgen05 GEMM pipeline time-out in an earlier backward pass (code %d)" % bwd_err)
+                raise _lib.PnbError("pnb200: tensor-core GEMM pipeline time-out in an earlier backward pass (code %d)" % bwd_err)
             self._valid_per_ray = max(self._valid_per_ray, n_valid / max(R, 1))
             if err == 9:
                 raise _lib.PnbOverflow("pnb200: an earlier render_full() produced %d valid samples, more than its shading workspace held "
                                        "(the extra samples were dropped); the workspace has been enlarged - render the frame again, or "
                                        "call check_errors() after each frame, or set opt.pnb_max_valid_per_ray" % n_valid)
             if err != 0:
-                raise _lib.PnbError("pnb200: tcgen05 pipeline time-out (code %d) in an earlier render_full()" % err)
+                raise _lib.PnbError("pnb200: tensor-core pipeline time-out (code %d) in an earlier render_full()" % err)
 
     # -------------------------------------------------------------------------------------------------
     def _run(self, campos, raydir, camrotc2w, near, far, bg_color, want_counters, t=None, frozen=False):
@@ -512,7 +512,7 @@ class NeuralPointsRayMarching(nn.Module):
             code = int(be[0].item())
             if code != 0:
                 be.zero_()
-                raise _lib.PnbError("pnb200: tcgen05 GEMM pipeline time-out in the backward pass (code %d)" % code)
+                raise _lib.PnbError("pnb200: tensor-core GEMM pipeline time-out in the backward pass (code %d)" % code)
         if self._err is not None:
             code = int(self._err[0].item())
             if code != 0:
@@ -524,7 +524,7 @@ class NeuralPointsRayMarching(nn.Module):
                                        "the workspace has been enlarged for the next call (or set opt.pnb_max_valid_per_ray)"
                                        % (n_valid, self._max_valid))
             if code != 0:
-                raise _lib.PnbError("pnb200: tcgen05 pipeline time-out (code %d)" % code)
+                raise _lib.PnbError("pnb200: tensor-core pipeline time-out (code %d)" % code)
 
     def _queue_status(self, q, dev):
         """Copies the device status of the call just issued to pinned memory behind its kernels (no host synchronisation); a later

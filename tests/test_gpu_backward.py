@@ -9,6 +9,7 @@ import torch
 
 from oracle import pipeline, shade_oracle
 from pointnerf_b200 import harness, scene
+from oracle import golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -24,8 +25,7 @@ def _close(a, ref, name, rtol=3e-4):
 def _close_points(a, ref, name, rtol=3e-4, max_outlier_frac=0.01, outlier_rtol=2e-2):
     """Per-point gradients of the tensor-core backward: its forward recompute carries the BF16x3 error, so ~1e-6 of the LeakyReLU
     units (those with a pre-activation within ~1e-5 of zero) get the other mask than the fp32 reference; each such unit changes the
-    gradient of ONE pair - i.e. of one point - by ~1/256 of that pair's contribution (csrc/backward.cu header; tools/bwd_diag2.py
-    lists them).  So: the strict tolerance on all points but <= 1 % of them (a few tens of flips per backward), and a bound on those."""
+    gradient of ONE pair - i.e. of one point - by ~1/256 of that pair's contribution (csrc/backward.cu header).  So: the strict tolerance on all points but <= 1 % of them (a few tens of flips per backward), and a bound on those."""
     a, ref = np.asarray(a, np.float64)[0], np.asarray(ref, np.float64).reshape(np.asarray(a).shape)[0]
     scale = max(np.abs(ref).max(), 1e-6)
     d = np.abs(a - ref).max(axis=-1)
@@ -43,10 +43,10 @@ def _forward(net, cfg, rays):
 @pytest.mark.parametrize("precision,bwd_fp32", [("bf16x3", 0), ("bf16x3", 1), ("bf16x3", 4), ("fp32", 0)])
 @pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1"])
 def test_gradients_match_reference_fixture(name, precision, bwd_fp32, golden_dir):
-    """bwd_fp32 = 0: every layer GEMM of the backward on the tensor cores (tcgen05, BF16x3; default); 4: the forward recompute on the
+    """bwd_fp32 = 0: every layer GEMM of the backward on the tensor cores (wgmma, BF16x3; default); 4: the forward recompute on the
     fp32 CUDA-core tiles (fp32-faithful LeakyReLU masks), dX / dW on the tensor cores; 1: everything on the fp32 tiles.  Modes 1 and 4
     meet the strict tolerance on every tensor; mode 0 on the MLP tensors and points_conf, and on all but a handful of points."""
-    fx = np.load(os.path.join(golden_dir, name + ".npz"))
+    fx = golden.load(golden_dir, name)
     cfg = scene.CONFIGS["tiny"]
     order = int(fx["agg_intrp_order"]) if "agg_intrp_order" in fx.files else 2       # tiny_order1: the reference run with --agg_intrp_order 1
     net, pts, opt = harness.build_model(cfg, DEV, SR=int(fx["SR"]), max_o=100000, pnb_precision=precision, pnb_bwd_fp32=bwd_fp32, agg_intrp_order=order)

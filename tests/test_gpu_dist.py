@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def test_nccl_train_render_grow_identical_across_ranks():
     n = torch.cuda.device_count()
     if n < 2:
-        pytest.skip("needs >= 2 GPUs (run with gpurun --gpus N)")
+        pytest.skip("needs >= 2 GPUs")
     s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", str(n), "--master-addr", "127.0.0.1",
                         "--master-port", str(port), os.path.join(ROOT, "tests", "dist_train_check.py")], capture_output=True, text=True, timeout=1200)

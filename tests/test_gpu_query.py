@@ -10,6 +10,7 @@ import torch
 from oracle import pipeline, query_oracle
 from pointnerf_b200 import harness, scene
 from pointnerf_b200.point_query import device_t_table_jitter
+from oracle import golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -70,7 +71,7 @@ def test_query_matches_oracle(name, side, over):
 
 @pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8"])
 def test_query_matches_reference_fixture(name, golden_dir):
-    fx = np.load(os.path.join(golden_dir, name + ".npz"))
+    fx = golden.load(golden_dir, name)
     cfg = scene.CONFIGS["tiny"]
     net, pts, opt = harness.build_model(cfg, DEV, SR=int(fx["SR"]), max_o=100000)
     out = _query_points(net, scene.make_rays(cfg, fx["pixels"]))

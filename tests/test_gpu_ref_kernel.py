@@ -1,16 +1,17 @@
 """GPU parity, integer path, pinned to an EXECUTION of the reference kernel.
 
-`oracle/_ref/query_worldcoords_cuda.so` is the reference's own, un-modified CUDA query extension
-(/root/reference/models/neural_points/cuda/query_worldcoords.{cpp,cu}, compiled for sm_100a by the committed recipe
-oracle/build_ref.py in the build container; it travels to the GPU box with the snapshot).  This test calls its
-`woord_query_grid_point_index` with the 18 arguments of /root/reference/models/neural_points/point_query.py:85-93 and the
-product (`libpnb200` through the drop-in `lighting_fast_querier.query_points`) on the same inputs.
+tests/golden/ref_kernel_<case>.npz hold what the reference's own, un-modified CUDA query extension
+(models/neural_points/cuda/query_worldcoords.{cpp,cu} of the reference, compiled for sm_90a by oracle/build_ref.py) returned on an H100
+when oracle/record_ref_kernel.py called its `woord_query_grid_point_index` with the 18 arguments of the reference's
+models/neural_points/point_query.py:85-93: the full ray mask and, for every kept ray (chair: a seeded sample of 2,500 of 9,216),
+the neighbour indices and world sample positions.  This test runs the product (`libpnb200` through the drop-in
+`lighting_fast_querier.query_points`) on the same inputs and compares.
 
 What can be asserted against a nondeterministic kernel (SURVEY 8a, Q1-Q3):
   * which occupied voxel wins occupancy slot 0 - and silently loses its points, query_worldcoords.cu:147 - depends on the
     order of the atomicAdd in claim_occ; the product drops the voxel of the lowest-index in-range point instead.  Samples whose
     (kernel_size+1)/2-shell neighbourhood contains either slot-0 voxel are EXCLUDED (counted, bounded); the reference's slot-0
-    voxel is recovered from the run itself: every point the reference misses must lie in ONE voxel.
+    voxel is recovered from the recorded run itself: every point the reference misses must lie in ONE voxel.
   * in-voxel point order depends on the atomics of fill_occ2pnts: neighbour SETS are compared (K nearest of the visited
     shells do not depend on the visiting order; exact distance ties would, none occur on these inputs).
 Everything else is bit-exact: ray mask, world sample positions, neighbour sets of every other sample.
@@ -21,23 +22,10 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import build_ref
-from pointnerf_b200 import harness, scene
+from oracle import record_ref_kernel as rec
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-_EXT = None
-
-
-def _ext():
-    global _EXT
-    if _EXT is None:
-        _EXT = build_ref.load_prebuilt()
-    if _EXT is None:
-        pytest.fail("oracle/_ref/query_worldcoords_cuda.so is missing: run `python -m oracle.build_ref` in the build container "
-                    "(it is git-ignored but travels with gpurun)")
-    return _EXT
 
 
 def _vox(p, lo, svs):
@@ -45,56 +33,40 @@ def _vox(p, lo, svs):
     return torch.floor((p - lo) / svs).to(torch.int64)
 
 
-def _run_both(name, pixels, over):
-    ext = _ext()
+def _run_both(case, golden_dir):
     dev = torch.device(DEV)
-    cfg = scene.CONFIGS[name]
-    net, pts, opt = harness.build_model(cfg, dev, **over)
-    rays = scene.make_rays(cfg, pixels)
-    r = {k: (v.to(dev) if isinstance(v, torch.Tensor) else v) for k, v in rays.items()}
-    raydir = r["raydir"].contiguous()
-    R = raydir.shape[1]
+    cfg, net, opt, r = rec.setup(case, dev)
+    ours = rec.product_query(cfg, net, r)
+    fx = np.load(os.path.join(golden_dir, "ref_kernel_%s.npz" % case))
+    R = int(fx["R"])
+    assert R == r["raydir"].shape[1]
+    ref_mask = torch.from_numpy(np.unpackbits(fx["mask_bits"])[:R].astype(bool)).to(dev)
+    ref = (torch.from_numpy(fx["pidx"]).to(dev), torch.from_numpy(fx["locw"]).to(dev), ref_mask, torch.from_numpy(fx["ray_idx"]).long().to(dev))
     querier = net.neural_points.querier
-    xyz = net.neural_points.xyz.detach().contiguous()
-    N = xyz.shape[0]
-    npts = torch.tensor([N], dtype=torch.int32, device=dev)
-    pix = r["pixel_idx"].to(torch.int32)
-    ours = querier.query_points(pix, None, xyz[None], npts, r["h"], r["w"], r["intrinsic"], np.float32(cfg.near),
-                                np.float32(cfg.far), raydir, r["campos"], r["camrotc2w"])
     gc = querier.last_grid_counters
     assert gc["overflow_o"] == 0 and gc["overflow_p"] == 0, "parity cases must not overflow max_o / P (Q3)"
     ranges_tensor, ranges_np, vsize_np, scaled_vdim_np = querier._hyper
-    t = querier._t_for(cfg.near, cfg.far, R, dev)
-    # ray generation of diff_ray_marching.py:386-388 as torch runs it on the device: one mul kernel, one add kernel
-    raypos = (r["campos"][:, None, None, :] + raydir[:, :, None, :] * t[None, None, :, None]).contiguous()
-    D = raypos.shape[2]
-    max_o = int(opt.max_o) if opt.max_o is not None else int(N)
+    max_o = int(opt.max_o) if opt.max_o is not None else int(net.neural_points.xyz.shape[0])
     assert gc["n_occ"] <= max_o
-    out = ext.woord_query_grid_point_index(
-        pix, raypos, xyz[None], npts, querier.kernel_size_tensor, querier.query_size_tensor, int(opt.SR), int(opt.K), R, D,
-        torch.as_tensor(scaled_vdim_np, device=dev), max_o, int(opt.P), float(querier.radius_limit_np), ranges_tensor.to(dev),
-        querier.scaled_vsize_tensor, 1024, 2)
-    torch.cuda.synchronize()
     lo = ranges_tensor[:3].to(dev)
     svs = querier.scaled_vsize_tensor
     dim = torch.as_tensor(scaled_vdim_np, device=dev).to(torch.int64)
-    return dict(cfg=cfg, opt=opt, ours=ours, ref=out, xyz=xyz, lo=lo, svs=svs, dim=dim, gc=gc, R=R,
+    return dict(cfg=cfg, opt=opt, ours=ours, ref=ref, xyz=net.neural_points.xyz.detach(), lo=lo, svs=svs, dim=dim, gc=gc, R=R,
                 layers=(int(opt.kernel_size[0]) + 1) // 2)
 
 
-def _compare(name, pixels, over, max_excluded_frac):
-    s = _run_both(name, pixels, over)
+def _compare(case, golden_dir, max_excluded_frac):
+    s = _run_both(case, golden_dir)
     o_pidx, o_locw, o_mask = s["ours"][0][0], s["ours"][2][0], s["ours"][4][0].reshape(-1) > 0
-    r_pidx, r_locw, r_mask = s["ref"][0][0], s["ref"][1][0], s["ref"][2][0].reshape(-1) > 0
+    r_pidx, r_locw, r_mask, r_rays = s["ref"]
     dim, lo, svs, xyz = s["dim"], s["lo"], s["svs"], s["xyz"]
 
-    # ---- rows of the rays both sides kept
-    both = o_mask & r_mask
-    row_o = (torch.cumsum(o_mask, 0) - 1)[both]
-    row_r = (torch.cumsum(r_mask, 0) - 1)[both]
+    # ---- rows of the recorded rays (all kept by the reference) that the product kept too
+    both = o_mask[r_rays]
+    row_o = (torch.cumsum(o_mask, 0) - 1)[r_rays[both]]
     a = torch.sort(o_pidx[row_o].to(torch.int64), dim=-1)[0]           # [Rb, SR, K]
-    b = torch.sort(r_pidx[row_r].to(torch.int64), dim=-1)[0]
-    la, lb = o_locw[row_o], r_locw[row_r]
+    b = torch.sort(r_pidx[both].to(torch.int64), dim=-1)[0]
+    la, lb = o_locw[row_o], r_locw[both]
     # sample positions: the reference leaves unfilled slots at 0 (get_shadingloc), so do we -> bit-exact everywhere
     assert torch.equal(la, lb), "world sample positions differ from the reference kernel"
 
@@ -128,53 +100,42 @@ def _compare(name, pixels, over, max_excluded_frac):
     n_excl = int(near.sum())
     assert n_excl <= max(27 * 24, max_excluded_frac * max(int(filled.sum()), 1)), "excluded %d samples" % n_excl
 
-    # ---- ray mask: equal except for rays whose every neighbour lies in a slot-0 voxel
+    # ---- ray mask (full frame): equal except for rays whose every neighbour lies in a slot-0 voxel
     md = o_mask != r_mask
     n_md = int(md.sum())
     assert n_md <= 4, "ray masks differ on %d rays" % n_md
     # the slot-order-free contract on the product's side: same sets AND the reference's K never exceeds ours
     print("[ref-kernel %s] rays %d hit %d/%d | samples compared %d identical, excluded %d (slot-0 voxels: ours %s, reference %s) | "
-          "mask diffs %d" % (name, s["R"], int(o_mask.sum()), int(r_mask.sum()), n_cmp, n_excl, oc.tolist(),
+          "mask diffs %d" % (case, s["R"], int(o_mask.sum()), int(r_mask.sum()), n_cmp, n_excl, oc.tolist(),
                              ref_cells[0].tolist() if ref_cells.shape[0] else None, n_md))
     return n_cmp
 
 
-def _block(cfg, x0, y0, w, h):
-    px, py = np.meshgrid(np.arange(x0, x0 + w), np.arange(y0, y0 + h))
-    return np.stack((px, py), -1).reshape(-1, 2).astype(np.float32)
+def test_ref_kernel_tiny_full_frame(golden_dir):
+    assert _compare("tiny_full", golden_dir, 0.05) > 1000
 
 
-def test_ref_kernel_tiny_full_frame():
-    cfg = scene.CONFIGS["tiny"]
-    assert _compare("tiny", None, {}, 0.05) > 1000
-
-
-def test_ref_kernel_chair():
-    cfg = scene.CONFIGS["chair_plumbing"]
-    assert _compare("chair_plumbing", scene.centre_patch(cfg, 96), {}, 0.02) > 1000
+def test_ref_kernel_chair(golden_dir):
+    assert _compare("chair_centre", golden_dir, 0.02) > 1000
 
 
 @pytest.mark.parametrize("sr", [24, 80])
-def test_ref_kernel_lego_chunk(sr):
+def test_ref_kernel_lego_chunk(sr, golden_dir):
     """One reference-sized chunk (48 x 48 = 2304 rays, run/train_ft.py:773) in the all-hit centre."""
-    cfg = scene.CONFIGS["lego_render"]
-    assert _compare("lego_render", scene.centre_patch(cfg, 48), dict(SR=sr), 0.01) > 10000
+    assert _compare("lego_centre_sr%d" % sr, golden_dir, 0.01) > 10000
 
 
-def test_ref_kernel_lego_silhouette():
+def test_ref_kernel_lego_silhouette(golden_dir):
     """A 96 x 24 strip through the limb of the shell (grazing hits, partial neighbourhoods, rays that miss)."""
-    cfg = scene.CONFIGS["lego_render"]
-    assert _compare("lego_render", _block(cfg, 400 + 240, 388, 96, 24), {}, 0.01) > 1000
+    assert _compare("lego_silhouette", golden_dir, 0.01) > 1000
 
 
-def test_ref_kernel_truck_chunk():
+def test_ref_kernel_truck_chunk(golden_dir):
     """N = 2 M, kernel_size 5 (three shells), grid 450^3: centre chunk and a corner strip through the limb."""
-    cfg = scene.CONFIGS["truck_8gpu"]
-    assert _compare("truck_8gpu", scene.centre_patch(cfg, 32), {}, 0.01) > 4000
-    assert _compare("truck_8gpu", _block(cfg, 860, 0, 100, 16), {}, 0.01) > 500
+    assert _compare("truck_centre", golden_dir, 0.01) > 4000
+    assert _compare("truck_corner", golden_dir, 0.01) > 500
 
 
-def test_ref_kernel_scannet_chunk():
+def test_ref_kernel_scannet_chunk(golden_dir):
     """N = 5 M inside a box, P = 30: every ray hits."""
-    cfg = scene.CONFIGS["scannet_8gpu"]
-    assert _compare("scannet_8gpu", scene.centre_patch(cfg, 24), {}, 0.01) > 1000
+    assert _compare("scannet_centre", golden_dir, 0.01) > 1000

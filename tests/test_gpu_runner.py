@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from pointnerf_b200 import checkpoint, harness, runner, scene
+from oracle import golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -37,7 +38,7 @@ def test_whole_image_equals_reference_chunk_loop():
 def test_reference_format_checkpoint_from_disk(golden_dir, tmp_path):
     """A `*_net_ray_marching.pth` file in the reference's layout (weights = the ones the reference module used for the
     tiny_opaque fixture) -> load_checkpoint -> drop-in forward() reproduces what the reference returned."""
-    fx = np.load(os.path.join(golden_dir, "tiny_opaque.npz"))
+    fx = golden.load(golden_dir, "tiny_opaque")
     cfg = scene.CONFIGS["tiny"]
     pts = scene.make_points(cfg)
     sd = {"aggregator." + k[4:]: torch.from_numpy(fx[k]) for k in fx.files if k.startswith("mlp.")}

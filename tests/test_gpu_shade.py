@@ -9,6 +9,7 @@ import torch
 
 from oracle import pipeline
 from pointnerf_b200 import harness, scene
+from oracle import golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -16,8 +17,8 @@ TOL = 1e-4
 
 
 def _prec(precision):
-    """bf16x3: the default (render_full / eval forward run the frozen-cloud pair kernel k_shade_tc8);
-    bf16x3-general: the general pair kernel k_shade_tc7 (what training steps run); fp32: the exact CUDA-core kernel."""
+    """bf16x3: the default (render_full / eval forward run the frozen-cloud pair kernel k_shade_wg<FROZEN>);
+    bf16x3-general: the general pair kernel k_shade_wg (what training steps run); fp32: the exact CUDA-core kernel."""
     if precision == "bf16x3-general":
         return dict(pnb_precision="bf16x3", pnb_frozen=0)
     return dict(pnb_precision=precision)
@@ -61,7 +62,7 @@ def test_render_matches_oracle(name, side, alpha_bias, over, precision):
 def test_forward_matches_reference_fixture(name, golden_dir, precision):
     """The drop-in NeuralPointsRayMarching.forward() output dict vs what the reference module itself returned
     (tiny_order1: the reference run with --agg_intrp_order 1, SURVEY 8(f) rank 4)."""
-    fx = np.load(os.path.join(golden_dir, name + ".npz"))
+    fx = golden.load(golden_dir, name)
     cfg = scene.CONFIGS["tiny"]
     order = int(fx["agg_intrp_order"]) if "agg_intrp_order" in fx.files else 2
     net, pts, opt = harness.build_model(cfg, DEV, SR=int(fx["SR"]), max_o=100000, agg_intrp_order=order, **_prec(precision))
@@ -91,7 +92,7 @@ def test_forward_matches_reference_fixture(name, golden_dir, precision):
 @pytest.mark.parametrize("name,side,over", [("tiny", 64, {}), ("chair_plumbing", 48, dict(SR=80)), ("lego_render", 40, {})])
 def test_render_order1_matches_oracle(name, side, over, precision):
     """agg_intrp_order = 1 (point_aggregators.py:573-599: alpha_branch on the K-aggregated feature) through render_full, all three
-    kernels (frozen / general tcgen05 pair kernels, fp32), against the oracle (itself pinned to the reference run of tiny_order1.npz)."""
+    kernels (frozen / general wgmma pair kernels, fp32), against the oracle (itself pinned to the reference run of tiny_order1.npz)."""
     cfg = scene.CONFIGS[name]
     net, pts, opt = harness.build_model(cfg, DEV, alpha_bias=3.0, agg_intrp_order=1, **_prec(precision), **over)
     rays = scene.make_rays(cfg, scene.centre_patch(cfg, side))
@@ -140,7 +141,7 @@ def test_render_lego_scale(precision):
 
 @pytest.mark.parametrize("name,side", [("truck_8gpu", 24), ("scannet_8gpu", 16)])
 def test_render_large_configs_chunk(name, side):
-    """BASELINE configs 4/5 sizes: rendered radiance of a chunk vs the oracle (default tcgen05 path)."""
+    """BASELINE configs 4/5 sizes: rendered radiance of a chunk vs the oracle (default wgmma path)."""
     cfg = scene.CONFIGS[name]
     net, pts, opt = harness.build_model(cfg, DEV, alpha_bias=3.0)
     rays = scene.make_rays(cfg, scene.centre_patch(cfg, side))
@@ -260,10 +261,9 @@ def test_frozen_table_follows_parameter_updates():
 
 
 @pytest.mark.parametrize("name,side,over", [("tiny", 64, {}), ("lego_render", 96, {}), ("lego_render", 64, dict(SR=80)), ("truck_8gpu", 48, {})])
-def test_deferred_last_epilogue_is_bit_identical(name, side, over):
-    """k_shade_tc8<DEFER = true> (default: the last epilogue of a tile is worked off in the gaps of the next tile, registers re-allocated
-    between the warpgroups) against the non-deferred form (pnb_dbg_flags bit 3): same arithmetic in the same order -> equal bits.
-    Several tiles per CTA (lego / truck patches) exercise the one-tile-late sigma hand-over between builder and epilogue warps."""
+def test_persistent_tile_loop_is_bit_identical(name, side, over):
+    """The pair and colour kernels on one CTA per 8 SMs (pnb_dbg_flags bit 3: many tiles per persistent CTA, the weight ring running
+    across tile boundaries) against the default launch (one CTA per SM): the same arithmetic per tile -> equal bits."""
     cfg = scene.CONFIGS[name]
     a, _, _ = harness.build_model(cfg, DEV, alpha_bias=3.0, **over)
     b, _, _ = harness.build_model(cfg, DEV, alpha_bias=3.0, pnb_dbg_flags=8, **over)
@@ -314,7 +314,7 @@ def test_probe_outputs_match_reference_fixture(golden_dir):
     """opt.prob == 1 (point-growing probe, run/train_ft.py:417-530): the extra per-ray outputs of the drop-in forward
     vs what the reference module returned (neural_points_volumetric_model.py:331-351)."""
     fx = np.load(os.path.join(golden_dir, "tiny_probe.npz"))
-    wfx = np.load(os.path.join(golden_dir, "tiny_opaque.npz"))
+    wfx = golden.load(golden_dir, "tiny_opaque")
     cfg = scene.CONFIGS["tiny"]
     net, pts, opt = harness.build_model(cfg, DEV, max_o=100000, prob=1)
     net.aggregator.load_state_dict({k[4:]: torch.from_numpy(wfx[k]) for k in wfx.files if k.startswith("mlp.")})

@@ -9,6 +9,7 @@ import torch
 
 from oracle import pipeline, query_oracle
 from pointnerf_b200 import scene
+from oracle import golden  # noqa: E402
 
 
 def brute_force(xyz, lo, svs, dim, ks, qs, P, r, campos, raydir, t, SR, K):
@@ -144,7 +145,7 @@ def test_oracle_edge_cases():
 def test_oracle_matches_reference_fixture(name, golden_dir):
     """oracle/pipeline.py (restated host logic + C query) == what the reference's own lighting_fast_querier class
     returned when the fixture was generated (oracle/make_golden.py)."""
-    fx = np.load(os.path.join(golden_dir, name + ".npz"))
+    fx = golden.load(golden_dir, name)
     cfg = scene.CONFIGS["tiny"]
     pts = scene.make_points(cfg)
     rays = scene.make_rays(cfg, fx["pixels"])

@@ -9,6 +9,7 @@ import torch
 
 from oracle import ref_shim, shade_oracle
 from pointnerf_b200 import scene
+from oracle import golden  # noqa: E402
 
 
 def _mlp_from(fx, prefix="mlp."):
@@ -17,7 +18,7 @@ def _mlp_from(fx, prefix="mlp."):
 
 @pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1"])
 def test_shade_oracle_matches_reference_fixture(name, golden_dir):
-    fx = np.load(os.path.join(golden_dir, name + ".npz"))
+    fx = golden.load(golden_dir, name)
     order = int(fx["agg_intrp_order"]) if "agg_intrp_order" in fx.files else 2
     cfg = scene.CONFIGS["tiny"]
     pts = scene.make_points(cfg)
@@ -46,7 +47,7 @@ def test_shade_oracle_matches_reference_fixture(name, golden_dir):
 
 
 def test_fill_invalid(golden_dir):
-    fx = np.load(os.path.join(golden_dir, "tiny_opaque.npz"))
+    fx = golden.load(golden_dir, "tiny_opaque")
     mask = torch.from_numpy(fx["ray_mask"]) > 0
     out = shade_oracle.fill_invalid(mask, torch.from_numpy(fx["coarse_raycolor"]), torch.from_numpy(fx["coarse_point_opacity"]),
                                     torch.from_numpy(fx["coarse_is_background"]), torch.zeros(int(mask.sum()), 3), torch.ones(3))
