@@ -207,7 +207,7 @@ enum {
     PNB_TC_FEW_CTAS = 2048      /* test of the persistent tile loop: one CTA per 8 SMs instead of one per SM (same results) */
 };
 /* Same contract as pnb_shade_forward; the MLPs run as wgmma tiles.  mlp->w[5] must be zero padded to 288 rows.
- * ws >= pnb_shade_tc_bytes(max_valid_samples).  d_err: device int32[>= 64], 0 on success, 9 if the query produced more valid
+ * ws >= pnb_shade_tc_bytes(max_valid_samples).  d_err: device int32[>= 1], 0 on success, 9 if the query produced more valid
  * samples than max_valid_samples (the extra samples are dropped: their sigma_rgb is zeroed, every other result is exact),
  * any other non-zero value = an internal pipeline time-out (a bounded 2-s mbarrier wait expired; results invalid). */
 size_t pnb_shade_tc_bytes(int max_valid_samples);

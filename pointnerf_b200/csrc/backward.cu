@@ -19,7 +19,7 @@
 // stops at ~1e-6 (tests/test_gpu_umma.py).  PNB_BWD_FP32_RECOMPUTE keeps the recompute on the fp32 CUDA-core tiles (fp32-faithful
 // masks, dX / dW still on the tensor cores); PNB_BWD_FP32_GEMM selects the hand-written fp32 CUDA-core tiles instead
 // (the parity reference of the tensor-core path; always used for the 128 -> 3 colour head).
-#include "common.cuh"
+#include "pair_inputs.cuh"
 #include "gemm_tc.cuh"
 
 namespace pnb {
@@ -251,112 +251,29 @@ struct BwdParams {
     const float* wa; const float* ba;
 };
 
-__device__ __forceinline__ void rot3b(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
-    ox = x * M[0] + y * M[1] + z * M[2];
-    oy = x * M[3] + y * M[4] + z * M[5];
-    oz = x * M[6] + y * M[7] + z * M[8];
-}
-__device__ __forceinline__ void rot3bT(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
-    ox = x * M[0] + y * M[3] + z * M[6];
-    oy = x * M[1] + y * M[4] + z * M[7];
-    oz = x * M[2] + y * M[5] + z * M[8];
-}
-__device__ __forceinline__ void w2persb(const pnb_shade_opts_t& o, float px, float py, float pz, float& xp, float& yp, float& zp) {
-    float sx = px - o.campos[0], sy = py - o.campos[1], sz = pz - o.campos[2];
-    const float* M = o.camrotc2w;
-    float xc = sx * M[0] + sy * M[3] + sz * M[6];
-    float yc = sx * M[1] + sy * M[4] + sz * M[7];
-    float zc = sx * M[2] + sy * M[5] + sz * M[8];
-    xp = xc / zc; yp = yc / zc; zp = zc;
-}
-
 // neighbour count of every valid sample (its exclusive prefix = the first packed row of the sample)
 __global__ void __launch_bounds__(256) k_bwd_counts(pnb_query_t q, int n_valid, uint32_t* __restrict__ nv) {
     const int vi = blockIdx.x * blockDim.x + threadIdx.x;
     if (vi < n_valid) nv[vi] = q.samp_nvalid[q.valid_list[vi]];
 }
-// One warp per valid sample, 4 lanes per pair row (same mapping as the fp32 forward kernel): dense block1 input.
+// One warp per valid sample, 4 lanes per pair row: the fp32 forward's row builder, writing the dense block1 input, the block3 extras
+// and the view PE to the recompute buffers.
 __global__ void __launch_bounds__(256) k_bwd_build(BwdParams p) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= p.n_valid) return;
     const pnb_query_t& q = p.q;
     const int vi = warp, k = lane >> 2, part = lane & 3;
-    uint32_t s = q.valid_list[vi];
-    const bool active = k < (int)q.samp_nvalid[s];          // the neighbours of a sample occupy its first slots
-    const long row = (long)p.pair_off[vi] + k;               // packed: only active lanes own a row
-    uint32_t pk = q.samp_ray[s];
-    int r = (int)(pk >> 7), j = (int)(pk & 127u);
-    int d = q.steps[(size_t)r * q.SR + j];
-    float t = q.t[(size_t)r * q.t_ray_stride + d];
-    float vx = q.raydir[3 * r], vy = q.raydir[3 * r + 1], vz = q.raydir[3 * r + 2];
-    float lx = raypos1(q.campos[0], vx, t), ly = raypos1(q.campos[1], vy, t), lz = raypos1(q.campos[2], vz, t);
-    int pidx = (active && k < q.K) ? q.cand_pidx[(size_t)s * q.K + k] : -1;
-    const bool valid = pidx >= 0;
-    const int pi = valid ? pidx : 0;
-    float ovx, ovy, ovz;
-    rot3b(p.o.Rw2c, vx, vy, vz, ovx, ovy, ovz);
+    const uint32_t s = q.valid_list[vi];
+    const long row = (long)p.pair_off[vi] + k;               // packed: only the sample's neighbours (its first slots) own a row
     float* cx = p.CX + (long)vi * 288;
-    if (lane < 12) {
-        int dd = lane >> 2, jj = lane & 3;
-        float sn, cs;
-        sincosf((dd == 0 ? ovx : dd == 1 ? ovy : ovz) * (float)(1 << jj), &sn, &cs);
-        cx[256 + lane] = sn;
-        cx[268 + lane] = cs;
-    }
-    if (lane < 8) cx[280 + lane] = 0.f;
-    float px = __ldg(&p.pts.xyz[3 * pi]), py = __ldg(&p.pts.xyz[3 * pi + 1]), pz = __ldg(&p.pts.xyz[3 * pi + 2]);
-    float dist[6];
-    dist[0] = px - lx; dist[1] = py - ly; dist[2] = pz - lz;
-    float xpp, ypp, zpp, xsp, ysp, zsp;
-    w2persb(p.o, px, py, pz, xpp, ypp, zpp);
-    w2persb(p.o, lx, ly, lz, xsp, ysp, zsp);
-    dist[3] = xpp * zpp - xsp * zsp; dist[4] = ypp * zpp - ysp * zsp; dist[5] = zpp - zsp;
-    float nrm = sqrtf(dist[0] * dist[0] + dist[1] * dist[1] + dist[2] * dist[2]);
-    float w = valid ? 1.0f / fmaxf(nrm, 1e-6f) : 0.f;
-    float wsum = part == 0 ? w : 0.f;
-    for (int o = 16; o > 0; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
-    w = w / fmaxf(wsum, 1e-8f);
-    float cf = __ldg(&p.pts.conf[pi]);
-    float cc = fminf(fmaxf(cf, 1e-4f), 1.0f);
-    if (part == 0 && valid) { p.wc[row] = w * cc; p.wn[row] = w; p.pidx[row] = pidx; p.row_samp[row] = vi; }
-    float d0, d1, d2;
-    rot3b(p.o.Rw2c, dist[0], dist[1], dist[2], d0, d1, d2);
-    dist[0] = d0; dist[1] = d1; dist[2] = d2;
-    float* xr = p.X1 + row * 288;
     float* er = p.X3 + row * 272 + 256;
-    if (valid) {
-        const float4* ep = (const float4*)&p.pts.emb[(size_t)pi * PNB_FEAT + part * 8];
-        float4 f0 = __ldg(ep), f1 = __ldg(ep + 1);
-        float f[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            int c = part * 8 + e;
-            xr[c] = f[e];
-#pragma unroll
-            for (int jj = 0; jj < 3; ++jj) {
-                float sn, cs;
-                sincosf(f[e] * (float)(1 << jj), &sn, &cs);
-                xr[32 + (c * 3 + jj) * 2] = sn;
-                xr[32 + (c * 3 + jj) * 2 + 1] = cs;
-            }
-        }
-        for (int i = part; i < 30; i += 4) {
-            int dd = i / 5, jj = i - dd * 5;
-            float sn, cs;
-            sincosf(dist[dd] * (float)(1 << jj), &sn, &cs);
-            xr[224 + i * 2] = sn;
-            xr[224 + i * 2 + 1] = cs;
-        }
-        if (part == 0) { xr[284] = 0.f; xr[285] = 0.f; xr[286] = 0.f; xr[287] = 0.f; }
-        if (part == 1) {
-            float ddx, ddy, ddz;
-            rot3b(p.o.Rw2c, __ldg(&p.pts.dir[3 * pi]), __ldg(&p.pts.dir[3 * pi + 1]), __ldg(&p.pts.dir[3 * pi + 2]), ddx, ddy, ddz);
-            er[0] = __ldg(&p.pts.color[3 * pi]); er[1] = __ldg(&p.pts.color[3 * pi + 1]); er[2] = __ldg(&p.pts.color[3 * pi + 2]);
-            er[3] = ddx - ovx; er[4] = ddy - ovy; er[5] = ddz - ovz;
-            er[6] = ddx * ovx + ddy * ovy + ddz * ovz;
-            for (int e = 7; e < 16; ++e) er[e] = 0.f;
-        }
-    }
+    const Fp32Pair pr = fp32_pair(q, p.pts, p.o, true, s, min((int)q.samp_nvalid[s], q.K), lane, cx + 256);
+    if (lane < 8) cx[280 + lane] = 0.f;
+    if (!pr.g.valid) return;
+    if (part == 0) { p.wc[row] = pr.wc; p.wn[row] = pr.wn; p.pidx[row] = pr.pidx; p.row_samp[row] = vi; }
+    fp32_pair_row(p.pts, p.o, pr, lane, p.X1 + row * 288, er);
+    if (part == 1)
+        for (int e = 7; e < 16; ++e) er[e] = 0.f;
 }
 
 // alpha branch + K-reduction forward (dense): one warp per sample.
@@ -380,9 +297,9 @@ __global__ void __launch_bounds__(256) k_bwd_reduce_fwd(BwdParams p) {
         }
         for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
         if (lane == 0 && p.o.agg_intrp_order != 1) {
-            float x = a + __ldg(p.ba) - 1.0f;
-            p.sp[r0 + k] = x > 20.f ? x : log1pf(expf(x));
-            p.sg[r0 + k] = 1.0f / (1.0f + expf(-x));
+            const float x = a + __ldg(p.ba);
+            p.sp[r0 + k] = softplus_m1(x);
+            p.sg[r0 + k] = 1.0f / (1.0f + expf(-(x - 1.0f)));   // its derivative
         }
     }
 #pragma unroll
@@ -395,9 +312,9 @@ __global__ void __launch_bounds__(256) k_bwd_reduce_fwd(BwdParams p) {
         for (int c = 0; c < 8; ++c) a = fmaf(hb[c], __ldg(&p.wa[lane + 32 * c]), a);
         for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
         if (lane == 0) {
-            float x = a + __ldg(p.ba) - 1.0f;
-            p.sp[r0] = x > 20.f ? x : log1pf(expf(x));
-            p.sg[r0] = 1.0f / (1.0f + expf(-x));
+            const float x = a + __ldg(p.ba);
+            p.sp[r0] = softplus_m1(x);
+            p.sg[r0] = 1.0f / (1.0f + expf(-(x - 1.0f)));
         }
     }
 }
@@ -571,13 +488,10 @@ __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* _
         if (d_color) { atomicAdd(&d_color[3 * pi], ge[0]); atomicAdd(&d_color[3 * pi + 1], ge[1]); atomicAdd(&d_color[3 * pi + 2], ge[2]); }
         if (d_dir) {
             // extras: (dir' - view')[3], <dir', view'>  with dir' = Rw2c * dir  ->  d dir = Rw2c^T (g[3:6] + g[6] * view')
-            uint32_t s = p.q.valid_list[p.row_samp[row]];
-            int r = (int)(p.q.samp_ray[s] >> 7);
-            float ovx, ovy, ovz;
-            rot3b(p.o.Rw2c, p.q.raydir[3 * r], p.q.raydir[3 * r + 1], p.q.raydir[3 * r + 2], ovx, ovy, ovz);
-            float gx = ge[3] + ge[6] * ovx, gy = ge[4] + ge[6] * ovy, gz = ge[5] + ge[6] * ovz;
+            const float3 ov = view_in_points(p.o, ray_dir(p.q, cand_ray(p.q, p.q.valid_list[p.row_samp[row]])));
+            float gx = ge[3] + ge[6] * ov.x, gy = ge[4] + ge[6] * ov.y, gz = ge[5] + ge[6] * ov.z;
             float ox, oy, oz;
-            rot3bT(p.o.Rw2c, gx, gy, gz, ox, oy, oz);
+            rot3T(p.o.Rw2c, gx, gy, gz, ox, oy, oz);
             atomicAdd(&d_dir[3 * pi], ox); atomicAdd(&d_dir[3 * pi + 1], oy); atomicAdd(&d_dir[3 * pi + 2], oz);
         }
         if (d_conf) atomicAdd(&d_conf[pi], dwc[row] * p.wn[row]);   // straight-through clamp (gradiant_clamp :722-724)
@@ -604,34 +518,15 @@ __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
         for (int j = 0; j < n; ++j) p.d_sigma_rgb[s0 + j] = make_float4(0.f, 0.f, 0.f, 0.f);
         return;
     }
-    const int SR = q.SR;
-    const float dx = q.raydir[3 * r], dy = q.raydir[3 * r + 1], dz = q.raydir[3 * r + 2];
-    const float* tr = q.t + (size_t)r * q.t_ray_stride;
-    const float* M = p.o.camrotc2w;
-    auto zcam = [&](float x, float y, float z) {
-        float sx = x - p.o.campos[0], sy = y - p.o.campos[1], sz = z - p.o.campos[2];
-        return sx * M[2] + sy * M[5] + sz * M[8];
-    };
-    auto zslot = [&](int j) {
-        if (j < n) {
-            float t = tr[q.steps[(size_t)r * SR + j]];
-            return zcam(raypos1(q.campos[0], dx, t), raypos1(q.campos[1], dy, t), raypos1(q.campos[2], dz, t));
-        }
-        return zcam(0.f, 0.f, 0.f);
-    };
-    const float vz = p.o.vsize_z;
+    const float3 dir = ray_dir(q, r);
     const float gR = p.d_ray_color[3 * r], gG = p.d_ray_color[3 * r + 1], gB = p.d_ray_color[3 * r + 2];
     // pass 1 (front to back): opacity, ray distance and transmittance of every candidate (local arrays, SR <= 128)
     float o_[PNB_MAX_SR], rd_[PNB_MAX_SR], T_[PNB_MAX_SR];
     float Tend;
     {
-        float cm = zslot(0), T = 1.0f;
+        float cm = slot_depth(q, p.o, r, n, 0, dir), T = 1.0f;
         for (int j = 0; j < n; ++j) {
-            float rd;
-            if (j + 1 < SR) { float zn = zslot(j + 1); float cmn = fmaxf(cm, zn); rd = cmn - cm; cm = cmn; } else rd = vz;
-            bool m = rd < 1e-8f;
-            if (p.o.raydist_mode_unit > 0) m = m || (rd > 2.0f * vz);
-            if (m) rd = vz;
+            const float rd = ray_dist_step(q, p.o, r, n, j, dir, cm);
             float o1 = 0.f;
             if (q.samp_nvalid[s0 + j] > 0) o1 = 1.0f - expf(-p.sigma_rgb[s0 + j].x * rd);
             o_[j] = o1; rd_[j] = rd; T_[j] = T;

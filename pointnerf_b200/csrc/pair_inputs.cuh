@@ -1,0 +1,228 @@
+// The reference's per-pair shading inputs, defined once for every kernel that builds or reads them: the fp32 forward
+// (k_shade_fwd), the tensor-core builders (k_shade_wg), the backward's recompute (k_bwd_build), and the kernels that need one
+// piece (k_color_wg, k_aux_outputs, k_composite, k_composite_bwd, k_bwd_scatter, k_bwd_reduce_fwd).
+//   sample position          diff_ray_marching.py:386
+//   dists / linear weights   point_aggregators.py:727-814, :421-429 (conf_coefficient: neural_points.py:706-717, :722-724)
+//   block3 extras            point_aggregators.py:560-571
+//   raw2out_density / _color point_aggregators.py:262-273
+//   ray distances            neural_points_volumetric_model.py:271-277
+// Under --fmad=true the FMA contraction follows the expression tree, so every kernel that inlines one of these expressions gets the
+// same bits: the backward's recompute agrees with the fp32 forward by construction.  What deliberately differs between the kernels
+// stays with them: the positional encoding (sincosf per frequency in the fp32 kernels, angle doubling on the tensor-core path) and
+// the order of the weight sum (32-lane butterfly, or the tensor-core path's segmented scan).
+#pragma once
+#include "common.cuh"
+
+namespace pnb {
+
+// v @ M^T (row vector times the transpose) == M v
+__device__ __forceinline__ void rot3(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
+    ox = x * M[0] + y * M[1] + z * M[2];
+    oy = x * M[3] + y * M[4] + z * M[5];
+    oz = x * M[6] + y * M[7] + z * M[8];
+}
+// M^T v
+__device__ __forceinline__ void rot3T(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
+    ox = x * M[0] + y * M[3] + z * M[6];
+    oy = x * M[1] + y * M[4] + z * M[7];
+    oz = x * M[2] + y * M[5] + z * M[8];
+}
+// neural_points.py:604-610 : xyz_c[j] = sum_i shift[i] * camrotc2w[i][j];  perspective (x / z, y / z, z)
+__device__ __forceinline__ void w2pers(const pnb_shade_opts_t& o, float px, float py, float pz, float& xp, float& yp, float& zp) {
+    float xc, yc, zc;
+    rot3T(o.camrotc2w, px - o.campos[0], py - o.campos[1], pz - o.campos[2], xc, yc, zc);
+    xp = xc / zc; yp = yc / zc; zp = zc;
+}
+// camera-space depth of a world position (z of w2pers)
+__device__ __forceinline__ float cam_depth(const pnb_shade_opts_t& o, float3 x) {
+    float xc, yc, zc;
+    rot3T(o.camrotc2w, x.x - o.campos[0], x.y - o.campos[1], x.z - o.campos[2], xc, yc, zc);
+    return zc;
+}
+
+// ------------------------------------------------------------------------------------------ samples
+__device__ __forceinline__ float3 ray_dir(const pnb_query_t& q, int r) {
+    return make_float3(q.raydir[3 * r], q.raydir[3 * r + 1], q.raydir[3 * r + 2]);
+}
+// ray parameter of slot j of ray r
+__device__ __forceinline__ float slot_t(const pnb_query_t& q, int r, int j) {
+    return q.t[(size_t)r * q.t_ray_stride + q.steps[(size_t)r * q.SR + j]];
+}
+__device__ __forceinline__ float3 ray_pos(const pnb_query_t& q, float3 dir, float t) {
+    return make_float3(raypos1(q.campos[0], dir.x, t), raypos1(q.campos[1], dir.y, t), raypos1(q.campos[2], dir.z, t));
+}
+// the ray of candidate sample s (samp_ray = ray << 7 | slot)
+__device__ __forceinline__ int cand_ray(const pnb_query_t& q, uint32_t s) { return (int)(q.samp_ray[s] >> 7); }
+struct CandSample {
+    float3 dir;   // its ray's direction
+    float3 pos;   // world position
+};
+__device__ __forceinline__ CandSample cand_sample(const pnb_query_t& q, uint32_t s) {
+    const uint32_t rj = q.samp_ray[s];
+    const int r = (int)(rj >> 7);
+    const float t = slot_t(q, r, (int)(rj & 127u));
+    CandSample c;
+    c.dir = ray_dir(q, r);
+    c.pos = ray_pos(q, c.dir, t);
+    return c;
+}
+// the view direction in the points' canonical frame (:526)
+__device__ __forceinline__ float3 view_in_points(const pnb_shade_opts_t& o, float3 dir) {
+    float3 v;
+    rot3(o.Rw2c, dir.x, dir.y, dir.z, v.x, v.y, v.z);
+    return v;
+}
+
+// ------------------------------------------------------------------------------------------ pairs
+// inverse-distance weight of a world offset (linear :424, :427), before the normalisation over the sample's neighbours
+__device__ __forceinline__ float inv_dist_weight(float dx, float dy, float dz) {
+    return 1.0f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-6f);
+}
+// :801-802
+__device__ __forceinline__ float norm_weight(float w, float wsum) { return w / fmaxf(wsum, 1e-8f); }
+// conf_coefficient: the forward value of gradiant_clamp (:722-724)
+__device__ __forceinline__ float conf_coef(float conf) { return fminf(fmaxf(conf, 1e-4f), 1.0f); }
+
+// Geometry of one (sample at l, point pidx) pair; pidx < 0 is an empty slot, read as point 0 with weight 0.
+struct PairGeom {
+    bool valid;
+    int pi;          // point index (0 for an empty slot)
+    float w;         // inverse-distance weight, not normalised
+    float cc;        // conf_coefficient
+    float dist[6];   // world offset + perspective terms (:782-784), rotated into the points' frame
+};
+__device__ __forceinline__ PairGeom pair_geom(const pnb_points_t& pts, const pnb_shade_opts_t& o, int pidx, float3 l) {
+    PairGeom g;
+    g.valid = pidx >= 0;
+    g.pi = g.valid ? pidx : 0;
+    const float px = __ldg(&pts.xyz[3 * g.pi]), py = __ldg(&pts.xyz[3 * g.pi + 1]), pz = __ldg(&pts.xyz[3 * g.pi + 2]);
+    const float dx = px - l.x, dy = py - l.y, dz = pz - l.z;
+    float xpp, ypp, zpp, xsp, ysp, zsp;
+    w2pers(o, px, py, pz, xpp, ypp, zpp);
+    w2pers(o, l.x, l.y, l.z, xsp, ysp, zsp);
+    g.dist[3] = xpp * zpp - xsp * zsp;
+    g.dist[4] = ypp * zpp - ysp * zsp;
+    g.dist[5] = zpp - zsp;
+    g.w = g.valid ? inv_dist_weight(dx, dy, dz) : 0.f;
+    g.cc = conf_coef(__ldg(&pts.conf[g.pi]));
+    rot3(o.Rw2c, dx, dy, dz, g.dist[0], g.dist[1], g.dist[2]);
+    return g;
+}
+// block3 extras of point pi seen along the view direction ov (points' frame): colour (3), dir - view (3), <dir, view> (1)
+__device__ __forceinline__ void point_extras(const pnb_points_t& pts, const pnb_shade_opts_t& o, int pi, float3 ov, float* ex) {
+    float ddx, ddy, ddz;
+    rot3(o.Rw2c, __ldg(&pts.dir[3 * pi]), __ldg(&pts.dir[3 * pi + 1]), __ldg(&pts.dir[3 * pi + 2]), ddx, ddy, ddz);
+    ex[0] = __ldg(&pts.color[3 * pi]); ex[1] = __ldg(&pts.color[3 * pi + 1]); ex[2] = __ldg(&pts.color[3 * pi + 2]);
+    ex[3] = ddx - ov.x; ex[4] = ddy - ov.y; ex[5] = ddz - ov.z;
+    ex[6] = ddx * ov.x + ddy * ov.y + ddz * ov.z;
+}
+
+// ------------------------------------------------------------------------------------------ outputs
+// raw2out_density: Softplus(a - 1), threshold 20
+__device__ __forceinline__ float softplus_m1(float a) {
+    const float x = a - 1.0f;
+    return x > 20.f ? x : log1pf(expf(x));
+}
+// raw2out_color: sigmoid scaled to (-0.001, 1.001)
+__device__ __forceinline__ float raw2out_color(float x) { return 1.0f / (1.0f + expf(-x)) * (1.0f + 2.0f * 0.001f) - 0.001f; }
+
+// ------------------------------------------------------------------------------------------ ray distances
+// camera depth of slot j of ray r (n filled slots); an unfilled slot holds the world origin (SURVEY a17)
+__device__ __forceinline__ float slot_depth(const pnb_query_t& q, const pnb_shade_opts_t& o, int r, int n, int j, float3 dir) {
+    if (j < n) return cam_depth(o, ray_pos(q, dir, slot_t(q, r, j)));
+    return cam_depth(o, make_float3(0.f, 0.f, 0.f));
+}
+// Ray distance of slot j: the step of the cumulative maximum of the slot depths to slot j + 1 (vsize_z for the last slot), replaced
+// by vsize_z below 1e-8 or, with raydist_mode_unit, above 2 vsize_z.  cm: the cumulative maximum up to slot j (start: slot_depth
+// of slot 0), advanced to slot j + 1.
+__device__ __forceinline__ float ray_dist_step(const pnb_query_t& q, const pnb_shade_opts_t& o, int r, int n, int j, float3 dir, float& cm) {
+    const float vz = o.vsize_z;
+    float rd;
+    if (j + 1 < q.SR) {
+        const float cmn = fmaxf(cm, slot_depth(q, o, r, n, j + 1, dir));
+        rd = cmn - cm;
+        cm = cmn;
+    } else {
+        rd = vz;
+    }
+    bool m = rd < 1e-8f;
+    if (o.raydist_mode_unit > 0) m = m || (rd > 2.0f * vz);
+    return m ? vz : rd;
+}
+
+// ------------------------------------------------------------------------------------------ fp32 row builder
+// The pair rows of the fp32 kernels (k_shade_fwd, k_bwd_build): one warp per sample, 4 lanes per row, lane = 4 * slot + part.
+// Two steps, so that a caller can store the row's scalars before the row itself (the backward's stores to global memory keep
+// their order, and the scalars need not stay live across the row):
+//   fp32_pair      the sample, the pair geometry and the weights; lanes 0-11 write the sample's view encoding PE4 (ori=True
+//                  layout, index d*4 + j: networks.py:183): sin to vpe[0..11], cos to vpe[12..23].  have: the warp has a sample s;
+//                  nk: slots k < nk are read from cand_pidx
+//   fp32_pair_row  for a non-empty slot, the row's four lanes write the 288 block1.0 inputs to xr (features (32), PE3 of the
+//                  features (192, index (c*3 + j)*2 + {sin, cos}), PE5 of the dists (60), 4 zeros); part 1 writes the 7 block3
+//                  extras to ex
+struct Fp32Pair {
+    PairGeom g;
+    int pidx;
+    float wn;     // normalised weight
+    float wc;     // weight * conf_coefficient (0 for an empty slot)
+    float3 ov;    // view direction in the points' frame
+};
+__device__ __forceinline__ Fp32Pair fp32_pair(const pnb_query_t& q, const pnb_points_t& pts, const pnb_shade_opts_t& o, bool have,
+                                              uint32_t s, int nk, int lane, float* vpe) {
+    const int k = lane >> 2, part = lane & 3;   // neighbour slot, quarter of the feature vector
+    CandSample cs = {};
+    Fp32Pair r;
+    r.pidx = -1;
+    if (have) {
+        cs = cand_sample(q, s);
+        if (k < nk) r.pidx = q.cand_pidx[(size_t)s * q.K + k];
+    }
+    r.ov = view_in_points(o, cs.dir);
+    if (lane < 12) {
+        const int dd = lane >> 2, jj = lane & 3;
+        float sn, cn;
+        sincosf((dd == 0 ? r.ov.x : dd == 1 ? r.ov.y : r.ov.z) * (float)(1 << jj), &sn, &cn);
+        vpe[lane] = sn;
+        vpe[12 + lane] = cn;
+    }
+    r.g = pair_geom(pts, o, r.pidx, cs.pos);
+    float wsum = part == 0 ? r.g.w : 0.f;       // sum over the 8 slots
+    for (int d = 16; d > 0; d >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, d);
+    r.wn = norm_weight(r.g.w, wsum);
+    r.wc = r.g.valid ? r.wn * r.g.cc : 0.f;
+    return r;
+}
+__device__ __forceinline__ void fp32_pair_row(const pnb_points_t& pts, const pnb_shade_opts_t& o, const Fp32Pair& r, int lane, float* xr,
+                                              float* ex) {
+    const int part = lane & 3;
+    const PairGeom& g = r.g;
+    // features: this lane's 8 channels + their PE (3 freqs)
+    const float4* ep = (const float4*)&pts.emb[(size_t)g.pi * PNB_FEAT + part * 8];
+    const float4 f0 = __ldg(ep), f1 = __ldg(ep + 1);
+    const float f[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const int c = part * 8 + e;
+        xr[c] = f[e];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            float sn, cn;
+            sincosf(f[e] * (float)(1 << j), &sn, &cn);
+            xr[32 + (c * 3 + j) * 2] = sn;
+            xr[32 + (c * 3 + j) * 2 + 1] = cn;
+        }
+    }
+    // distance PE (5 freqs): 30 (d, j) pairs split over the 4 lanes
+    const float dist[6] = {g.dist[0], g.dist[1], g.dist[2], g.dist[3], g.dist[4], g.dist[5]};
+    for (int i = part; i < 30; i += 4) {
+        const int dd = i / 5, jj = i - dd * 5;
+        float sn, cn;
+        sincosf(dist[dd] * (float)(1 << jj), &sn, &cn);
+        xr[224 + i * 2] = sn;
+        xr[224 + i * 2 + 1] = cn;
+    }
+    if (part == 0) { xr[284] = 0.f; xr[285] = 0.f; xr[286] = 0.f; xr[287] = 0.f; }
+    if (part == 1) point_extras(pts, o, g.pi, r.ov, ex);
+}
+
+}  // namespace pnb

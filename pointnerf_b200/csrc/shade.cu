@@ -14,7 +14,7 @@
 // Tile = 8 valid samples x 8 neighbour slots = 64 (sample,k) pair rows; one warp builds one sample's rows.
 // Activations never leave shared memory; weights (W^T, zero padded to multiples of 16 rows) stream from L2
 // through a cp.async double buffer.
-#include "common.cuh"
+#include "pair_inputs.cuh"
 
 namespace pnb {
 
@@ -152,24 +152,6 @@ __device__ __forceinline__ void dense8(const float* __restrict__ in, int sin_, f
     __syncthreads();
 }
 
-__device__ __forceinline__ void rot3(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
-    // v @ M^T  (row vector times transpose) == M * v
-    ox = x * M[0] + y * M[1] + z * M[2];
-    oy = x * M[3] + y * M[4] + z * M[5];
-    oz = x * M[6] + y * M[7] + z * M[8];
-}
-
-__device__ __forceinline__ void w2pers(const pnb_shade_opts_t& o, float px, float py, float pz, float& xp, float& yp,
-                                       float& zp) {
-    // neural_points.py:604-610 : xyz_c[j] = sum_i shift[i] * camrotc2w[i][j]
-    float sx = px - o.campos[0], sy = py - o.campos[1], sz = pz - o.campos[2];
-    const float* M = o.camrotc2w;
-    float xc = sx * M[0] + sy * M[3] + sz * M[6];
-    float yc = sx * M[1] + sy * M[4] + sz * M[7];
-    float zc = sx * M[2] + sy * M[5] + sz * M[8];
-    xp = xc / zc; yp = yc / zc; zp = zc;
-}
-
 __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     ShadeSmem& sm = *reinterpret_cast<ShadeSmem*>(smem_raw);
@@ -184,98 +166,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
             const int vi = tile * TS + warp;
             const int k = lane >> 2, part = lane & 3;  // neighbour slot, quarter of the feature vector
             const int row = warp * PNB_MAX_K + k;
-            uint32_t s = 0xffffffffu;
-            int pidx = -1;
-            float lx = 0.f, ly = 0.f, lz = 0.f, vx = 0.f, vy = 0.f, vz = 0.f;
-            if (vi < n_valid) {
-                s = q.valid_list[vi];
-                uint32_t pk = q.samp_ray[s];
-                int r = (int)(pk >> 7), j = (int)(pk & 127u);
-                int d = q.steps[(size_t)r * q.SR + j];
-                float t = q.t[(size_t)r * q.t_ray_stride + d];
-                vx = q.raydir[3 * r]; vy = q.raydir[3 * r + 1]; vz = q.raydir[3 * r + 2];
-                lx = raypos1(q.campos[0], vx, t); ly = raypos1(q.campos[1], vy, t); lz = raypos1(q.campos[2], vz, t);
-                if (k < q.K) pidx = q.cand_pidx[(size_t)s * q.K + k];
-            }
-            if (lane == 0) sm.samp[warp] = s;
-            const bool valid = pidx >= 0;
-            const int pi = valid ? pidx : 0;
-            // view direction in the points' canonical frame + its encoding (per sample; lanes 0..11 do the PE)
-            float ovx, ovy, ovz;
-            rot3(p.o.Rw2c, vx, vy, vz, ovx, ovy, ovz);
-            if (lane < 3) sm.view[warp][lane] = lane == 0 ? ovx : lane == 1 ? ovy : ovz;
-            if (lane < 12) {  // index d*4 + j  (networks.py:183), ori=True layout: [p, sin(12), cos(12)]
-                int dd = lane >> 2, jj = lane & 3;
-                float v = (dd == 0 ? ovx : dd == 1 ? ovy : ovz) * (float)(1 << jj);
-                float sn, cs;
-                sincosf(v, &sn, &cs);
-                sm.view[warp][3 + lane] = sn;
-                sm.view[warp][15 + lane] = cs;
-            }
-            // geometry of this pair
-            float px = __ldg(&p.pts.xyz[3 * pi]), py = __ldg(&p.pts.xyz[3 * pi + 1]), pz = __ldg(&p.pts.xyz[3 * pi + 2]);
-            float dist[6];
-            dist[0] = px - lx; dist[1] = py - ly; dist[2] = pz - lz;
-            float xpp, ypp, zpp, xsp, ysp, zsp;
-            w2pers(p.o, px, py, pz, xpp, ypp, zpp);
-            w2pers(p.o, lx, ly, lz, xsp, ysp, zsp);
-            dist[3] = xpp * zpp - xsp * zsp;  // point_aggregators.py:782-784
-            dist[4] = ypp * zpp - ysp * zsp;
-            dist[5] = zpp - zsp;
-            float nrm = sqrtf(dist[0] * dist[0] + dist[1] * dist[1] + dist[2] * dist[2]);
-            float w = valid ? 1.0f / fmaxf(nrm, 1e-6f) : 0.f;       // linear :424, :427
-            float wsum = w;                                          // sum over the 8 slots (lanes with part == 0)
-            wsum = part == 0 ? wsum : 0.f;
-            for (int o = 16; o > 0; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
-            w = w / fmaxf(wsum, 1e-8f);                              // :801-802
-            float cf = __ldg(&p.pts.conf[pi]);
-            float cc = fminf(fmaxf(cf, 1e-4f), 1.0f);                // gradiant_clamp forward value :722-724
-            if (part == 0) sm.wc[row] = valid ? w * cc : 0.f;
-            // rotate world offsets into the canonical frame (:526)
-            float d0, d1, d2;
-            rot3(p.o.Rw2c, dist[0], dist[1], dist[2], d0, d1, d2);
-            dist[0] = d0; dist[1] = d1; dist[2] = d2;
+            const bool have = vi < n_valid;
+            const uint32_t s = have ? q.valid_list[vi] : 0xffffffffu;
             float* xr = &sm.X[row * XS];
-            if (valid) {
-                // features: this lane's 8 channels + their PE (3 freqs): index (c*3 + j)*2 + {sin,cos}
-                const float4* ep = (const float4*)&p.pts.emb[(size_t)pi * PNB_FEAT + part * 8];
-                float4 f0 = __ldg(ep), f1 = __ldg(ep + 1);
-                float f[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    int c = part * 8 + e;
-                    xr[c] = f[e];
-#pragma unroll
-                    for (int j = 0; j < 3; ++j) {
-                        float sn, cs;
-                        sincosf(f[e] * (float)(1 << j), &sn, &cs);
-                        xr[32 + (c * 3 + j) * 2] = sn;
-                        xr[32 + (c * 3 + j) * 2 + 1] = cs;
-                    }
-                }
-                // distance PE (5 freqs): 30 (d, j) pairs split over the 4 lanes
-                for (int i = part; i < 30; i += 4) {
-                    int dd = i / 5, jj = i - dd * 5;
-                    float sn, cs;
-                    sincosf(dist[dd] * (float)(1 << jj), &sn, &cs);
-                    xr[224 + i * 2] = sn;
-                    xr[224 + i * 2 + 1] = cs;
-                }
-                if (part == 0) { xr[284] = 0.f; xr[285] = 0.f; xr[286] = 0.f; xr[287] = 0.f; }
-                if (part == 1) {  // block3 extras (:560-571)
-                    float cr = __ldg(&p.pts.color[3 * pi]), cg = __ldg(&p.pts.color[3 * pi + 1]), cb = __ldg(&p.pts.color[3 * pi + 2]);
-                    float ddx, ddy, ddz;
-                    rot3(p.o.Rw2c, __ldg(&p.pts.dir[3 * pi]), __ldg(&p.pts.dir[3 * pi + 1]), __ldg(&p.pts.dir[3 * pi + 2]), ddx, ddy, ddz);
-                    sm.E[row][0] = cr; sm.E[row][1] = cg; sm.E[row][2] = cb;
-                    sm.E[row][3] = ddx - ovx; sm.E[row][4] = ddy - ovy; sm.E[row][5] = ddz - ovz;
-                    sm.E[row][6] = ddx * ovx + ddy * ovy + ddz * ovz;
-                    sm.E[row][7] = 0.f;
-                }
+            if (lane == 0) sm.samp[warp] = s;
+            const Fp32Pair pr = fp32_pair(q, p.pts, p.o, have, s, q.K, lane, &sm.view[warp][3]);
+            if (lane < 3) sm.view[warp][lane] = lane == 0 ? pr.ov.x : lane == 1 ? pr.ov.y : pr.ov.z;
+            if (part == 0) sm.wc[row] = pr.wc;
+            if (pr.g.valid) {
+                fp32_pair_row(p.pts, p.o, pr, lane, xr, sm.E[row]);
             } else {
                 for (int c = part; c < 288; c += 4) xr[c] = 0.f;
                 if (part == 1)
-                    for (int e = 0; e < 8; ++e) sm.E[row][e] = 0.f;
+                    for (int e = 0; e < 7; ++e) sm.E[row][e] = 0.f;
             }
+            if (part == 1) sm.E[row][7] = 0.f;
         }
         __syncthreads();
         // ------------------------------------------------------------------ phase B: per-pair MLPs
@@ -296,10 +201,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
             for (int c = part; c < 256; c += 4) a = fmaf(sm.X[row * XS + c], __ldg(&wa[c]), a);
             a += __shfl_xor_sync(0xffffffffu, a, 1);
             a += __shfl_xor_sync(0xffffffffu, a, 2);
-            if (part == 0) {
-                float x = a + __ldg(&p.mlp.b[4][0]) - 1.0f;           // raw2out_density: Softplus(x - 1), threshold 20
-                sm.alpha[row] = x > 20.f ? x : log1pf(expf(x));
-            }
+            if (part == 0) sm.alpha[row] = softplus_m1(a + __ldg(&p.mlp.b[4][0]));
         }
         __syncthreads();
         // ------------------------------------------------------------------ phase C: K-reduction -> colour input
@@ -331,17 +233,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
                     const float* wa = p.mlp.w[4];
                     float a = 0.f;
                     for (int c = 0; c < 256; ++c) a = fmaf(sm.H[tid * HS + c], __ldg(&wa[c]), a);
-                    const float x = a + __ldg(&p.mlp.b[4][0]) - 1.0f;
-                    sg = x > 20.f ? x : log1pf(expf(x));
+                    sg = softplus_m1(a + __ldg(&p.mlp.b[4][0]));
                 } else {
 #pragma unroll
                     for (int k = 0; k < PNB_MAX_K; ++k) sg += sm.alpha[tid * PNB_MAX_K + k] * sm.wc[tid * PNB_MAX_K + k];
                 }
                 float4 o4;
                 o4.x = sg;
-                o4.y = 1.0f / (1.0f + expf(-B1[tid * XS + 0])) * (1.0f + 2.0f * 0.001f) - 0.001f;  // raw2out_color
-                o4.z = 1.0f / (1.0f + expf(-B1[tid * XS + 1])) * (1.0f + 2.0f * 0.001f) - 0.001f;
-                o4.w = 1.0f / (1.0f + expf(-B1[tid * XS + 2])) * (1.0f + 2.0f * 0.001f) - 0.001f;
+                o4.y = raw2out_color(B1[tid * XS + 0]);
+                o4.z = raw2out_color(B1[tid * XS + 1]);
+                o4.w = raw2out_color(B1[tid * XS + 2]);
                 p.sigma_rgb[s] = o4;
             }
         }
@@ -376,37 +277,11 @@ __global__ void __launch_bounds__(128) k_composite(CompositeParams p) {
     }
     const int n = q.nsamp[r];
     const uint32_t s0 = q.samp_off[r];
-    const float dx = q.raydir[3 * r], dy = q.raydir[3 * r + 1], dz = q.raydir[3 * r + 2];
-    const float* tr = q.t + (size_t)r * q.t_ray_stride;
-    const float* M = p.o.camrotc2w;
-    // camera-space depth of a world position (z of w2pers); unfilled slots hold the world origin (SURVEY a17)
-    auto zcam = [&](float x, float y, float z) {
-        float sx = x - p.o.campos[0], sy = y - p.o.campos[1], sz = z - p.o.campos[2];
-        return sx * M[2] + sy * M[5] + sz * M[8];
-    };
-    auto zslot = [&](int j) {
-        if (j < n) {
-            float t = tr[q.steps[(size_t)r * SR + j]];
-            return zcam(raypos1(q.campos[0], dx, t), raypos1(q.campos[1], dy, t), raypos1(q.campos[2], dz, t));
-        }
-        return zcam(0.f, 0.f, 0.f);
-    };
-    const float vz = p.o.vsize_z;
-    float cm = zslot(0);  // cummax so far
+    const float3 dir = ray_dir(q, r);
+    float cm = slot_depth(q, p.o, r, n, 0, dir);  // cummax so far
     float T = 1.0f, cr = 0.f, cg = 0.f, cb = 0.f;
     for (int j = 0; j < SR; ++j) {
-        float rd;
-        if (j + 1 < SR) {
-            float zn = zslot(j + 1);
-            float cmn = fmaxf(cm, zn);
-            rd = cmn - cm;
-            cm = cmn;
-        } else {
-            rd = vz;
-        }
-        bool m = rd < 1e-8f;
-        if (p.o.raydist_mode_unit > 0) m = m || (rd > 2.0f * vz);
-        if (m) rd = vz;
+        float rd = ray_dist_step(q, p.o, r, n, j, dir, cm);
         float sg = 0.f, rr = 0.f, gg = 0.f, bb = 0.f;
         bool valid = false;
         if (j < n && q.samp_nvalid[s0 + j] > 0) {
@@ -454,31 +329,29 @@ __global__ void __launch_bounds__(128) k_aux_outputs(AuxParams p) {
     const int rr = (int)(idx / SR), j = (int)(idx - (long long)rr * SR);
     const int r = (int)p.rows[rr];
     const int n = q.nsamp[r];
-    float lx = 0.f, ly = 0.f, lz = 0.f;
+    float3 l = make_float3(0.f, 0.f, 0.f);
     const int32_t* pid = nullptr;
     if (j < n) {
-        const float t = q.t[(size_t)r * q.t_ray_stride + q.steps[(size_t)r * SR + j]];
-        lx = raypos1(q.campos[0], q.raydir[3 * r], t); ly = raypos1(q.campos[1], q.raydir[3 * r + 1], t); lz = raypos1(q.campos[2], q.raydir[3 * r + 2], t);
+        const float t = slot_t(q, r, j);
+        l = ray_pos(q, ray_dir(q, r), t);
         pid = q.cand_pidx + (size_t)(q.samp_off[r] + j) * K;
     }
     float w[PNB_MAX_K], wsum = 0.f;
-    const float c_first = fminf(fmaxf(__ldg(p.conf), 1e-4f), 1.0f);
+    const float c_first = conf_coef(__ldg(p.conf));
     float* cc = p.cc + (size_t)idx * K;
     for (int k = 0; k < K; ++k) {
         const int pi = pid ? pid[k] : -1;
         w[k] = 0.f;
         float c = c_first;
         if (pi >= 0) {
-            const float dx = __ldg(&p.xyz[3 * pi]) - lx, dy = __ldg(&p.xyz[3 * pi + 1]) - ly, dz = __ldg(&p.xyz[3 * pi + 2]) - lz;
-            w[k] = 1.0f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-6f);
-            c = fminf(fmaxf(__ldg(&p.conf[pi]), 1e-4f), 1.0f);
+            w[k] = inv_dist_weight(__ldg(&p.xyz[3 * pi]) - l.x, __ldg(&p.xyz[3 * pi + 1]) - l.y, __ldg(&p.xyz[3 * pi + 2]) - l.z);
+            c = conf_coef(__ldg(&p.conf[pi]));
         }
         wsum += w[k];
         cc[k] = c;
     }
-    const float inv = fmaxf(wsum, 1e-8f);
     float* wo = p.weight + (size_t)idx * K;
-    for (int k = 0; k < K; ++k) wo[k] = w[k] / inv;
+    for (int k = 0; k < K; ++k) wo[k] = norm_weight(w[k], wsum);
     // blend_weight = opacity * exclusive cumprod(1 - opacity + 1e-10)   (diff_ray_marching.py:536-541)
     const float* op = p.opacity + (size_t)r * SR;
     float T = 1.0f;

@@ -16,7 +16,7 @@
 //   A = A_hi + A_lo, W = W_hi + W_lo (bf16 each);   D = A_hi*W_hi + A_lo*W_hi + A_hi*W_lo    (3 MMAs per k-step)
 // Weight images are pre-packed per K = 16 step in the wgmma operand layout (pnb_mlp_pack) and streamed L2 -> shared memory with
 // cp.async.bulk (TMA engine) through a 4-stage mbarrier ring.
-#include "common.cuh"
+#include "pair_inputs.cuh"
 #include "wgmma.cuh"
 
 namespace pnb {
@@ -55,20 +55,6 @@ struct ShadeTcParams {
     const float* pre;            // FROZEN: per-point hoisted layer-1 pre-activation [N][256] (k_point_pre)
 };
 
-__device__ __forceinline__ void rot3t(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
-    ox = x * M[0] + y * M[1] + z * M[2];
-    oy = x * M[3] + y * M[4] + z * M[5];
-    oz = x * M[6] + y * M[7] + z * M[8];
-}
-__device__ __forceinline__ void w2pers_t(const pnb_shade_opts_t& o, float px, float py, float pz, float& xp, float& yp, float& zp) {
-    float sx = px - o.campos[0], sy = py - o.campos[1], sz = pz - o.campos[2];
-    const float* M = o.camrotc2w;
-    float xc = sx * M[0] + sy * M[3] + sz * M[6];
-    float yc = sx * M[1] + sy * M[4] + sz * M[7];
-    float zc = sx * M[2] + sy * M[5] + sz * M[8];
-    xp = xc / zc; yp = yc / zc; zp = zc;
-}
-
 // sin/cos of x*2^j, j = 0..NF-1: one accurate sincosf + angle doubling (abs error < 1e-6 after 4 doublings; the
 // fp32 kernel keeps NF independent sincosf calls).  out[2j] = sin, out[2j+1] = cos  (networks.py:175-190 layout).
 template <int NF>
@@ -94,11 +80,6 @@ __device__ __forceinline__ void store_chunk8_a1(SmemT& sm, int r, int kb, int k8
     *reinterpret_cast<uint4*>(sm.a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-// One pair row of the block1 operand (gather, distance weights, PE by angle doubling, hi/lo split -> shared memory),
-// its block3 extras operand and its weight*conf factor.  PART 2: the whole row (v3 / v5: one builder thread per row);
-// PART 0 / 1: the two halves of a row for the v6 pipeline (two builder threads per row):
-//   part 0 = operand columns 0..151   (raw features, PE of features 0..19)
-//   part 1 = operand columns 152..287 (PE of features 20..31, PE of the 6 distances), extras operand, weight*conf
 // Sum of v over the lanes st .. st+cnt-1 of the warp (cnt <= 8; every lane calls it, lanes outside any segment pass st = lane,
 // cnt = 1).  The order of the additions depends on cnt only, not on where the segment sits in the warp.
 __device__ __forceinline__ float seg_scan8(float v, int lane, int st) {          // inclusive scan within the segment
@@ -113,100 +94,74 @@ __device__ __forceinline__ float seg_sum8(float v, int lane, int st, int cnt) {
     return __shfl_sync(0xffffffffu, seg_scan8(v, lane, st), st + cnt - 1);
 }
 
-// PACKED = false: row = 8 * (sample in tile) + neighbour slot, 16 samples per tile (rows of empty slots are zero).
-// PACKED = true (v7): the caller has packed only the valid (sample, neighbour) pairs into the rows: row `row` is neighbour `pk` of
-// valid sample `pvi` (pvi < 0: unused row), and the rows of that sample are lanes pst .. pst+pcnt-1 of this warp.
-template <int PART, bool PACKED = false, class SmemT>
-__device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& p, int tile, int t, int row, int n_valid, int pvi = -1,
-                                                int pk = 0, int pst = 0, int pcnt = 1) {
+// One pair row of the layer-1 operand (gather, distance weights, PE by angle doubling, hi/lo split -> shared memory).  The caller
+// has packed only the valid (sample, neighbour) pairs into the rows: row `row` is neighbour `pk` of valid sample `pvi` (pvi < 0:
+// unused row), and the rows of that sample are lanes pst .. pst+pcnt-1 of this warp.  Two builder threads per row:
+//   part 0 = operand columns 0..151   (raw features, PE of features 0..19)
+//   part 1 = operand columns 152..287 (PE of features 20..31, PE of the 6 distances), extras operand, weight*conf
+// FROZEN (part 1 only, one builder thread per row): the feature columns come from the per-point table, so the row is part 1
+// without the feature PE and with the distance PE at operand columns 0..63 (K blocks 0, 1); it also records the row's point.
+template <int PART, bool FROZEN, class SmemT>
+__device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& p, int row, int n_valid, int pvi, int pk, int pst, int pcnt) {
     using namespace tc;
-    constexpr bool P0 = PART != 1, P1 = PART != 0;
-    constexpr int G_LO = P0 ? 0 : 5, G_HI = P1 ? 8 : 5;      // feature groups (4 features each) whose PE this part builds
+    static_assert(PART == 0 || PART == 1, "two parts per row");
+    static_assert(!FROZEN || PART == 1, "the frozen row is a part-1 row");
+    constexpr bool P0 = PART == 0, P1 = PART == 1;
+    constexpr int G_LO = P0 ? 0 : 5, G_HI = (P1 && !FROZEN) ? 8 : 5;   // feature groups (4 features each) whose PE this part builds
+    constexpr int DCOL = FROZEN ? 0 : 224;                              // first operand column of the distance PE
+    constexpr int C_LO = P1 && !FROZEN ? 19 : 0, C_HI = P0 ? 19 : FROZEN ? 8 : 36;   // 16-byte chunks (column / 8) of this part
     const pnb_query_t& q = p.q;
-    const int k = PACKED ? pk : (row & 7);
-    const int vi = PACKED ? pvi : tile * (TM / PNB_MAX_K) + (row >> 3);
     int pidx = -1;
-    float lx = 0.f, ly = 0.f, lz = 0.f, vx = 0.f, vy = 0.f, vz = 0.f;
-    if (vi >= 0 && vi < n_valid) {
-        uint32_t s = q.valid_list[vi];
-        if (P1) {
-            uint32_t pk = q.samp_ray[s];
-            int r = (int)(pk >> 7), j = (int)(pk & 127u);
-            int d = q.steps[(size_t)r * q.SR + j];
-            float tt = q.t[(size_t)r * q.t_ray_stride + d];
-            vx = q.raydir[3 * r]; vy = q.raydir[3 * r + 1]; vz = q.raydir[3 * r + 2];
-            lx = raypos1(q.campos[0], vx, tt); ly = raypos1(q.campos[1], vy, tt); lz = raypos1(q.campos[2], vz, tt);
-        }
-        if (k < q.K) pidx = q.cand_pidx[(size_t)s * q.K + k];
+    CandSample cs = {};
+    if (pvi >= 0 && pvi < n_valid) {
+        const uint32_t s = q.valid_list[pvi];
+        if (P1) cs = cand_sample(q, s);
+        if (pk < q.K) pidx = q.cand_pidx[(size_t)s * q.K + pk];
     }
+    if (FROZEN) sm.prow[row] = pidx;
     const bool valid = pidx >= 0;
     const int pi = valid ? pidx : 0;
-    float dist[6];
-    float ovx = 0.f, ovy = 0.f, ovz = 0.f;
+    PairGeom g;
+    float3 ov;
     if (P1) {
-        rot3t(p.o.Rw2c, vx, vy, vz, ovx, ovy, ovz);
-        float px = __ldg(&p.pts.xyz[3 * pi]), py = __ldg(&p.pts.xyz[3 * pi + 1]), pz = __ldg(&p.pts.xyz[3 * pi + 2]);
-        dist[0] = px - lx; dist[1] = py - ly; dist[2] = pz - lz;
-        float xpp, ypp, zpp, xsp, ysp, zsp;
-        w2pers_t(p.o, px, py, pz, xpp, ypp, zpp);
-        w2pers_t(p.o, lx, ly, lz, xsp, ysp, zsp);
-        dist[3] = xpp * zpp - xsp * zsp; dist[4] = ypp * zpp - ysp * zsp; dist[5] = zpp - zsp;
-        float nrm = sqrtf(dist[0] * dist[0] + dist[1] * dist[1] + dist[2] * dist[2]);
-        float w = valid ? 1.0f / fmaxf(nrm, 1e-6f) : 0.f;
-        float wsum = w;
-        if (PACKED) {
-            wsum = seg_sum8(w, row & 31, pst, pcnt);
-        } else {                               // 8 consecutive lanes = the 8 rows of one sample
-            wsum += __shfl_xor_sync(0xffffffffu, wsum, 1);
-            wsum += __shfl_xor_sync(0xffffffffu, wsum, 2);
-            wsum += __shfl_xor_sync(0xffffffffu, wsum, 4);
-        }
-        w = w / fmaxf(wsum, 1e-8f);
-        float cf = __ldg(&p.pts.conf[pi]);
-        sm.wc[t % SmemT::NWC][row] = valid ? w * fminf(fmaxf(cf, 1e-4f), 1.0f) : 0.f;
-        float d0, d1, d2;
-        rot3t(p.o.Rw2c, dist[0], dist[1], dist[2], d0, d1, d2);
-        dist[0] = d0; dist[1] = d1; dist[2] = d2;
+        ov = view_in_points(p.o, cs.dir);
+        g = pair_geom(p.pts, p.o, pidx, cs.pos);
+        const float wsum = seg_sum8(g.w, row & 31, pst, pcnt);   // every lane takes part in the shuffles
+        sm.wc[row] = valid ? norm_weight(g.w, wsum) * g.cc : 0.f;
     }
     float ex[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (valid) {
         const float4* ep = (const float4*)&p.pts.emb[(size_t)pi * PNB_FEAT];
 #pragma unroll
-        for (int g = G_LO; g < G_HI; ++g) {    // 4 features per step
-            float4 fv = __ldg(ep + g);
+        for (int gi = G_LO; gi < G_HI; ++gi) {  // 4 features per step
+            float4 fv = __ldg(ep + gi);
             float f[4] = {fv.x, fv.y, fv.z, fv.w};
             float pe[24];
 #pragma unroll
             for (int e = 0; e < 4; ++e) pe_doubling<3>(f[e], pe + e * 6);
-            const int col = 32 + 24 * g;
+            const int col = 32 + 24 * gi;
 #pragma unroll
             for (int c = 0; c < 3; ++c) store_chunk8_a1(sm, row, (col + 8 * c) >> 5, (col + 8 * c) & 31, pe + 8 * c);
         }
         if (P0) {
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {      // raw features, 8 per chunk (re-read: L1 hit)
-                float4 a = __ldg(ep + 2 * g), b = __ldg(ep + 2 * g + 1);
+            for (int gi = 0; gi < 4; ++gi) {    // raw features, 8 per chunk (re-read: L1 hit)
+                float4 a = __ldg(ep + 2 * gi), b = __ldg(ep + 2 * gi + 1);
                 float f8[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-                store_chunk8_a1(sm, row, 0, 8 * g, f8);
+                store_chunk8_a1(sm, row, 0, 8 * gi, f8);
             }
         }
         if (P1) {
-            float dp[60];
+            float dp[64];
 #pragma unroll
-            for (int e = 0; e < 6; ++e) pe_doubling<5>(dist[e], dp + 10 * e);
-            float z4[8] = {dp[56], dp[57], dp[58], dp[59], 0.f, 0.f, 0.f, 0.f};
+            for (int e = 0; e < 6; ++e) pe_doubling<5>(g.dist[e], dp + 10 * e);
+            dp[60] = dp[61] = dp[62] = dp[63] = 0.f;
 #pragma unroll
-            for (int c = 0; c < 7; ++c) store_chunk8_a1(sm, row, (224 + 8 * c) >> 5, (224 + 8 * c) & 31, dp + 8 * c);
-            store_chunk8_a1(sm, row, 8, 24, z4);
-            float ddx, ddy, ddz;
-            rot3t(p.o.Rw2c, __ldg(&p.pts.dir[3 * pi]), __ldg(&p.pts.dir[3 * pi + 1]), __ldg(&p.pts.dir[3 * pi + 2]), ddx, ddy, ddz);
-            ex[0] = __ldg(&p.pts.color[3 * pi]); ex[1] = __ldg(&p.pts.color[3 * pi + 1]); ex[2] = __ldg(&p.pts.color[3 * pi + 2]);
-            ex[3] = ddx - ovx; ex[4] = ddy - ovy; ex[5] = ddz - ovz;
-            ex[6] = ddx * ovx + ddy * ovy + ddz * ovz;
+            for (int c = 0; c < 8; ++c) store_chunk8_a1(sm, row, (DCOL + 8 * c) >> 5, (DCOL + 8 * c) & 31, dp + 8 * c);
+            point_extras(p.pts, p.o, pi, ov, ex);
         }
     } else {
         float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        constexpr int C_LO = P0 ? 0 : 19, C_HI = P1 ? 36 : 19;   // 16-byte chunks: column / 8
         for (int c = C_LO; c < C_HI; ++c) store_chunk8_a1(sm, row, c >> 2, (c & 3) * 8, z8);
     }
     if (P1) {   // block3 extras operand [128 x 16]: chunk 0 = extras, chunk 1 = 0
@@ -214,10 +169,10 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
 #pragma unroll
         for (int i = 0; i < 4; ++i) split_bf16x2(ex[2 * i], ex[2 * i + 1], h[i], l[i]);
         uint32_t off = tc::xe_offset(row, 0);
-        *reinterpret_cast<uint4*>(sm.xe_hi[t & 1] + off) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint4*>(sm.xe_lo[t & 1] + off) = make_uint4(l[0], l[1], l[2], l[3]);
-        *reinterpret_cast<uint4*>(sm.xe_hi[t & 1] + off + 128) = make_uint4(0u, 0u, 0u, 0u);
-        *reinterpret_cast<uint4*>(sm.xe_lo[t & 1] + off + 128) = make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(sm.xe_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
+        *reinterpret_cast<uint4*>(sm.xe_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
+        *reinterpret_cast<uint4*>(sm.xe_hi + off + 128) = make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(sm.xe_lo + off + 128) = make_uint4(0u, 0u, 0u, 0u);
     }
 }
 // ------------------------------------------------------------------------------------------ weight packing
@@ -485,73 +440,6 @@ __global__ void __launch_bounds__(256) k_point_pre(const float* __restrict__ emb
         if (n0 + i < N) pre[(size_t)(n0 + i) * 256 + c] = acc[i] + bc;
 }
 
-// One pair row of the frozen pipeline: the PE5(dists) K blocks of the layer-1 operand (operand columns 224..287 -> blocks 0, 1),
-// the block3 extras operand, weight*conf and the row's point index.  Same arithmetic as build_pair_part<PART 1, PACKED>.
-template <class SmemT>
-__device__ __forceinline__ void build_pair_frozen(SmemT& sm, const ShadeTcParams& p, int t, int row, int n_valid, int pvi, int pk, int pst, int pcnt) {
-    using namespace tc;
-    const pnb_query_t& q = p.q;
-    int pidx = -1;
-    float lx = 0.f, ly = 0.f, lz = 0.f, vx = 0.f, vy = 0.f, vz = 0.f;
-    if (pvi >= 0 && pvi < n_valid) {
-        const uint32_t s = q.valid_list[pvi];
-        const uint32_t sr = q.samp_ray[s];
-        const int r = (int)(sr >> 7), j = (int)(sr & 127u);
-        const int d = q.steps[(size_t)r * q.SR + j];
-        const float tt = q.t[(size_t)r * q.t_ray_stride + d];
-        vx = q.raydir[3 * r]; vy = q.raydir[3 * r + 1]; vz = q.raydir[3 * r + 2];
-        lx = raypos1(q.campos[0], vx, tt); ly = raypos1(q.campos[1], vy, tt); lz = raypos1(q.campos[2], vz, tt);
-        if (pk < q.K) pidx = q.cand_pidx[(size_t)s * q.K + pk];
-    }
-    const bool valid = pidx >= 0;
-    const int pi = valid ? pidx : 0;
-    sm.prow[t & 1][row] = pidx;
-    float dist[6];
-    float ovx, ovy, ovz;
-    rot3t(p.o.Rw2c, vx, vy, vz, ovx, ovy, ovz);
-    const float px = __ldg(&p.pts.xyz[3 * pi]), py = __ldg(&p.pts.xyz[3 * pi + 1]), pz = __ldg(&p.pts.xyz[3 * pi + 2]);
-    dist[0] = px - lx; dist[1] = py - ly; dist[2] = pz - lz;
-    float xpp, ypp, zpp, xsp, ysp, zsp;
-    w2pers_t(p.o, px, py, pz, xpp, ypp, zpp);
-    w2pers_t(p.o, lx, ly, lz, xsp, ysp, zsp);
-    dist[3] = xpp * zpp - xsp * zsp; dist[4] = ypp * zpp - ysp * zsp; dist[5] = zpp - zsp;
-    const float nrm = sqrtf(dist[0] * dist[0] + dist[1] * dist[1] + dist[2] * dist[2]);
-    float w = valid ? 1.0f / fmaxf(nrm, 1e-6f) : 0.f;
-    const float wsum = seg_sum8(w, row & 31, pst, pcnt);
-    w = w / fmaxf(wsum, 1e-8f);
-    const float cf = __ldg(&p.pts.conf[pi]);
-    sm.wc[t & 1][row] = valid ? w * fminf(fmaxf(cf, 1e-4f), 1.0f) : 0.f;
-    float d0, d1, d2;
-    rot3t(p.o.Rw2c, dist[0], dist[1], dist[2], d0, d1, d2);
-    dist[0] = d0; dist[1] = d1; dist[2] = d2;
-    float ex[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (valid) {
-        float dp[64];
-#pragma unroll
-        for (int e = 0; e < 6; ++e) pe_doubling<5>(dist[e], dp + 10 * e);
-        dp[60] = dp[61] = dp[62] = dp[63] = 0.f;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) store_chunk8_a1(sm, row, c >> 2, (c & 3) * 8, dp + 8 * c);
-        float ddx, ddy, ddz;
-        rot3t(p.o.Rw2c, __ldg(&p.pts.dir[3 * pi]), __ldg(&p.pts.dir[3 * pi + 1]), __ldg(&p.pts.dir[3 * pi + 2]), ddx, ddy, ddz);
-        ex[0] = __ldg(&p.pts.color[3 * pi]); ex[1] = __ldg(&p.pts.color[3 * pi + 1]); ex[2] = __ldg(&p.pts.color[3 * pi + 2]);
-        ex[3] = ddx - ovx; ex[4] = ddy - ovy; ex[5] = ddz - ovz;
-        ex[6] = ddx * ovx + ddy * ovy + ddz * ovz;
-    } else {
-        const float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int c = 0; c < 8; ++c) store_chunk8_a1(sm, row, c >> 2, (c & 3) * 8, z8);
-    }
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) split_bf16x2(ex[2 * i], ex[2 * i + 1], h[i], l[i]);
-    const uint32_t off = tc::xe_offset(row, 0);
-    *reinterpret_cast<uint4*>(sm.xe_hi[t & 1] + off) = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(sm.xe_lo[t & 1] + off) = make_uint4(l[0], l[1], l[2], l[3]);
-    *reinterpret_cast<uint4*>(sm.xe_hi[t & 1] + off + 128) = make_uint4(0u, 0u, 0u, 0u);
-    *reinterpret_cast<uint4*>(sm.xe_lo[t & 1] + off + 128) = make_uint4(0u, 0u, 0u, 0u);
-}
-
 // =====================================================================================================================
 // k_shade_wg: the pair MLPs of the packed 128-row tiles (a tile is four 32-row quadrants, each holding whole samples back to back,
 // only their valid neighbours: 99 % of the rows carry a pair on the lego frame).  One persistent CTA per SM, 256 threads = two
@@ -571,16 +459,15 @@ constexpr int NSTAGE = 4;
 constexpr int YLD = 260;                  // fp32 row stride of the last-epilogue buffer: lane = row float4 reads are conflict-free
 constexpr int KS_FROZEN0 = 14;            // first K step of the frozen layer 1 (operand columns 224..287 of block1.0)
 struct Smem {
-    static constexpr int NWC = 1;
     unsigned char a_hi[tc::NKB_MAX * tc::ABLK];   // layer operand; a_hi + a_lo also hold the fp32 [128 x YLD] rows of the last epilogue
     unsigned char a_lo[tc::NKB_MAX * tc::ABLK];
     unsigned char b[NSTAGE][tc::STEP];
-    unsigned char xe_hi[1][tc::XE];
-    unsigned char xe_lo[1][tc::XE];
-    float wc[1][tc::TM];
-    int prow[1][tc::TM];                  // FROZEN: point index of every row (-1: unused row)
+    unsigned char xe_hi[tc::XE];
+    unsigned char xe_lo[tc::XE];
+    float wc[tc::TM];
+    int prow[tc::TM];                     // FROZEN: point index of every row (-1: unused row)
     float alpha_part[2][tc::TM];
-    uint32_t qhead[1][4], qfirst[1][4], qtotal[1][4];
+    uint32_t qhead[4], qfirst[4], qtotal[4];   // per quadrant: segment heads, first packed position, rows
     uint64_t bar_full[NSTAGE], bar_empty[NSTAGE];
 };
 static_assert(tc::TM * YLD * 4 <= 2 * tc::NKB_MAX * tc::ABLK, "last-epilogue rows exceed the operand region");
@@ -624,7 +511,7 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
     if (tid == 0) ring.prologue();
 
     const uint32_t a_hi0 = smem_u32(sm.a_hi) + (uint32_t)wgi * 4096u, a_lo0 = smem_u32(sm.a_lo) + (uint32_t)wgi * 4096u;
-    const uint32_t xe_hi0 = smem_u32(sm.xe_hi[0]) + (uint32_t)wgi * 2048u, xe_lo0 = smem_u32(sm.xe_lo[0]) + (uint32_t)wgi * 2048u;
+    const uint32_t xe_hi0 = smem_u32(sm.xe_hi) + (uint32_t)wgi * 2048u, xe_lo0 = smem_u32(sm.xe_lo) + (uint32_t)wgi * 2048u;
     const uint32_t b0 = smem_u32(sm.b[0]);
     const int r0 = 64 * wgi + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);   // fragment: rows r0, r0 + 8; columns 8j + cq, +1
     float* ybuf = reinterpret_cast<float*>(sm.a_hi);
@@ -649,11 +536,11 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
                 const int total = __shfl_sync(0xffffffffu, incl, 31);
                 const QuadRow qr = quad_row(head, total, lane);
                 const int cj = __shfl_sync(0xffffffffu, c, qr.j);
-                if (lane == 0 && part == 0) { sm.qhead[0][qw] = head; sm.qfirst[0][qw] = first; sm.qtotal[0][qw] = (uint32_t)total; }
+                if (lane == 0 && part == 0) { sm.qhead[qw] = head; sm.qfirst[qw] = first; sm.qtotal[qw] = (uint32_t)total; }
                 const int pvi = qr.live ? (int)p.vorder[first + qr.j] : -1;
-                if (FROZEN) build_pair_frozen(sm, p, 0, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else if (part == 0) build_pair_part<0, true>(sm, p, tile, 0, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else build_pair_part<1, true>(sm, p, tile, 0, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                if (FROZEN) build_pair_part<1, true>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else if (part == 0) build_pair_part<0, false>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else build_pair_part<1, false>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
             }
             fence_proxy_async();
             named_bar_sync(1, hw::NTHR);
@@ -689,8 +576,8 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
             const float* pre0 = nullptr;
             const float* pre1 = nullptr;
             if (FROZEN && l == 0) {                                  // unused rows (prow < 0): any finite values
-                pre0 = p.pre + (size_t)max(sm.prow[0][r0], 0) * 256;
-                pre1 = p.pre + (size_t)max(sm.prow[0][r0 + 8], 0) * 256;
+                pre0 = p.pre + (size_t)max(sm.prow[r0], 0) * 256;
+                pre1 = p.pre + (size_t)max(sm.prow[r0 + 8], 0) * 256;
             }
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
@@ -728,10 +615,10 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
         named_bar_sync(1, hw::NTHR);
         {
             const int qd = warp & 3, half = warp >> 2, row = qd * 32 + lane;      // columns 128 half .. 128 half + 127 of the row
-            const QuadRow qr = quad_row(sm.qhead[0][qd], (int)sm.qtotal[0][qd], lane);
-            const int sidx = qr.live ? (int)p.vorder[sm.qfirst[0][qd] + qr.j] : 0;
+            const QuadRow qr = quad_row(sm.qhead[qd], (int)sm.qtotal[qd], lane);
+            const int sidx = qr.live ? (int)p.vorder[sm.qfirst[qd] + qr.j] : 0;
             const bool swrite = qr.is_end && sidx < n_valid;
-            const float wrow = sm.wc[0][row];
+            const float wrow = sm.wc[row];
             const float* yr = ybuf + row * hw::YLD + 128 * half;
             float apart = 0.f;
 #pragma unroll 1
@@ -749,8 +636,7 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
             if (half == 0) {
                 // sigma = softplus(alpha dot product - 1): order 2 per neighbour, weighted sum over the sample's rows; order 1: `a` is
                 // already the sample's value (its last row).  The two column halves are added in a fixed order: deterministic.
-                const float a = (sm.alpha_part[0][row] + sm.alpha_part[1][row]) + __ldg(p.ba) - 1.0f;
-                const float sp = a > 20.f ? a : log1pf(expf(a));
+                const float sp = softplus_m1((sm.alpha_part[0][row] + sm.alpha_part[1][row]) + __ldg(p.ba));
                 const float zz = O1 ? sp : seg_scan8(sp * wrow, lane, qr.st);
                 if (swrite) p.sigma[sidx] = zz;
             }
@@ -840,9 +726,8 @@ __global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
             for (int i = 0; i < 32; ++i) pe[i] = 0.f;
             if (vi < n_valid) {
                 const uint32_t s = q.valid_list[vi];
-                const int r = (int)(q.samp_ray[s] >> 7);
-                float ov[3];
-                rot3t(p.o.Rw2c, q.raydir[3 * r], q.raydir[3 * r + 1], q.raydir[3 * r + 2], ov[0], ov[1], ov[2]);
+                const float3 v = view_in_points(p.o, ray_dir(q, cand_ray(q, s)));
+                const float ov[3] = {v.x, v.y, v.z};
 #pragma unroll
                 for (int d = 0; d < 3; ++d) {     // ori=True layout: sin block (d*4+j) then cos block
                     float sc[8];
@@ -938,9 +823,9 @@ __global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
                             const uint32_t s = q.valid_list[vi];
                             float4 o4;
                             o4.x = p.sigma[vi];
-                            o4.y = 1.0f / (1.0f + expf(-(d[h][0] + __ldg(p.b3)))) * (1.0f + 2.0f * 0.001f) - 0.001f;
-                            o4.z = 1.0f / (1.0f + expf(-(d[h][1] + __ldg(p.b3 + 1)))) * (1.0f + 2.0f * 0.001f) - 0.001f;
-                            o4.w = 1.0f / (1.0f + expf(-(d[h][2] + __ldg(p.b3 + 2)))) * (1.0f + 2.0f * 0.001f) - 0.001f;
+                            o4.y = raw2out_color(d[h][0] + __ldg(p.b3));
+                            o4.z = raw2out_color(d[h][1] + __ldg(p.b3 + 1));
+                            o4.w = raw2out_color(d[h][2] + __ldg(p.b3 + 2));
                             p.sigma_rgb[s] = o4;
                         }
                     }

@@ -361,8 +361,8 @@ def _init_state(mod):
     if mod.precision not in ("bf16x3", "fp32"):
         raise NotImplementedError("pnb200: pnb_precision=%r (bf16x3 | fp32)" % mod.precision)
     # pnb_frozen: 1 (default) = calls that need no gradient (rendering, evaluation) run the frozen-cloud pair kernel
-    # (k_shade_tc8: the point-only inputs of block1.0 hoisted into a per-point table, rebuilt when points_embeding or
-    # block1.0 change); 0 = always the general kernel (k_shade_tc7), which is what training steps use in either case.
+    # (k_shade_wg<FROZEN>: the point-only inputs of block1.0 hoisted into a per-point table, rebuilt when points_embeding or
+    # block1.0 change); 0 = always the general kernel (k_shade_wg), which is what training steps use in either case.
     mod.frozen_ok = bool(int(getattr(opt, "pnb_frozen", 1)))
     mod.dbg_flags = int(getattr(opt, "pnb_dbg_flags", 0)) | int(os.environ.get("PNB_DBG_FLAGS_DEFAULT", "0"))   # (env: kernel experiments under the test-suite)
     mod.last = None
@@ -478,7 +478,7 @@ class NeuralPointsRayMarching(nn.Module):
                 self._tc_ws = None
                 self._tc_ws = torch.empty(nb, dtype=torch.uint8, device=dev)
             if self._err is None or self._err.device != dev:
-                self._err = torch.zeros(512, dtype=torch.int32, device=dev)   # [0] status, [2:64] cycle counters, [64:] per-CTA cycles (int64)
+                self._err = torch.zeros(1, dtype=torch.int32, device=dev)     # status of the tensor-core pipeline
             else:
                 self._err[:1].zero_()
             flags = _lib.TC_PAIRS | _lib.TC_COLOR | (self.dbg_flags << 8)
