@@ -137,6 +137,10 @@ typedef struct {
     const float* dir;   /* [N,3] */
     const float* conf;  /* [N]   */
     int32_t N;
+    const float* rw2c;  /* [N][9] per-point Rw2c, row-major, or NULL (every point uses pnb_shade_opts_t.Rw2c).  Edited / composed
+                         * scenes (run/editing.py) give each point its own frame: a pair's dists and dir use its point's frame, the
+                         * view direction of a sample (PE(view) and every pair's extras) the frame of its slot-0 neighbour
+                         * (point_aggregators.py:491-496, :506, :526, :566).  No gradient flows to it. */
 } pnb_points_t;
 
 int pnb_version(void);

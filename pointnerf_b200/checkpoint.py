@@ -3,7 +3,7 @@
 The reference writes, per saved iteration (`/root/reference/models/base_model.py:85-103`):
   `{epoch}_net_ray_marching.pth`  = `net_ray_marching.state_dict()` (after unwrapping `nn.DataParallel`): flat dict
       neural_points.xyz [N,3] | neural_points.points_embeding [1,N,32] | neural_points.points_conf [1,N,1] |
-      neural_points.points_dir [1,N,3] | neural_points.points_color [1,N,3] | (neural_points.eulers, neural_points.Rw2c) |
+      neural_points.points_dir [1,N,3] | neural_points.points_color [1,N,3] | (neural_points.eulers, neural_points.Rw2c [3,3] or [N,3,3]) |
       aggregator.{block1.0,block1.2,block3.0,block3.2,alpha_branch.0,color_branch.0,.2,.4,.6}.{weight,bias}
   `{epoch}_states.pth`            = free-form dict of runner state (`epoch_count`, `total_steps`, optimiser states ...)
 and reads them back with `NeuralPoints.__init__(checkpoint=...)` (`models/neural_points/neural_points.py:242-288`) and
@@ -67,6 +67,11 @@ def validate(sd, opt=None):
         c = int(getattr(opt, "point_features_dim", sd["neural_points.points_embeding"].shape[-1]))
         if sd["neural_points.points_embeding"].shape[-1] != c:
             raise CheckpointError("points_embeding has %d channels, opt.point_features_dim=%d" % (sd["neural_points.points_embeding"].shape[-1], c))
+    if "neural_points.Rw2c" in sd:
+        # one rotation for the whole cloud, or one per point (a checkpoint saved after an edit, run/editing.py)
+        R = sd["neural_points.Rw2c"]
+        if tuple(R.shape) not in ((3, 3), (n, 3, 3)) or R.dtype != torch.float32:
+            raise CheckpointError("neural_points.Rw2c has shape %s / %s; needs fp32 [3,3] or [N,3,3] for N=%d" % (tuple(R.shape), R.dtype, n))
     if "neural_points.eulers" in sd:
         raise NotImplementedError("pnb200: per-point euler rotations (neural_points.eulers) are outside the shipped hot path")
     unknown = [k for k in sd if not (k in POINT_KEYS or k in OPTIONAL_POINT_KEYS or k.startswith("aggregator."))]

@@ -258,6 +258,7 @@ __global__ void __launch_bounds__(256) k_bwd_counts(pnb_query_t q, int n_valid, 
 }
 // One warp per valid sample, 4 lanes per pair row: the fp32 forward's row builder, writing the dense block1 input, the block3 extras
 // and the view PE to the recompute buffers.
+template <bool PP>
 __global__ void __launch_bounds__(256) k_bwd_build(BwdParams p) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= p.n_valid) return;
@@ -267,11 +268,11 @@ __global__ void __launch_bounds__(256) k_bwd_build(BwdParams p) {
     const long row = (long)p.pair_off[vi] + k;               // packed: only the sample's neighbours (its first slots) own a row
     float* cx = p.CX + (long)vi * 288;
     float* er = p.X3 + row * 272 + 256;
-    const Fp32Pair pr = fp32_pair(q, p.pts, p.o, true, s, min((int)q.samp_nvalid[s], q.K), lane, cx + 256);
+    const Fp32Pair pr = fp32_pair<PP>(q, p.pts, p.o, true, s, min((int)q.samp_nvalid[s], q.K), lane, cx + 256);
     if (lane < 8) cx[280 + lane] = 0.f;
     if (!pr.g.valid) return;
     if (part == 0) { p.wc[row] = pr.wc; p.wn[row] = pr.wn; p.pidx[row] = pr.pidx; p.row_samp[row] = vi; }
-    fp32_pair_row(p.pts, p.o, pr, lane, p.X1 + row * 288, er);
+    fp32_pair_row<PP>(p.pts, p.o, pr, lane, p.X1 + row * 288, er);
     if (part == 1)
         for (int e = 7; e < 16; ++e) er[e] = 0.f;
 }
@@ -458,6 +459,7 @@ __global__ void __launch_bounds__(128) k_dw_small(const float* __restrict__ X, l
 }
 
 // Scatter to the points: embedding (through PE), colour, dir, conf.  4 lanes per pair row.
+template <bool PP>
 __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* __restrict__ dwc, float* __restrict__ d_emb,
                                                      float* __restrict__ d_color, float* __restrict__ d_dir, float* __restrict__ d_conf) {
     const long gt = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -487,11 +489,13 @@ __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* _
         const float* ge = p.G2 + row * 272 + 256;
         if (d_color) { atomicAdd(&d_color[3 * pi], ge[0]); atomicAdd(&d_color[3 * pi + 1], ge[1]); atomicAdd(&d_color[3 * pi + 2], ge[2]); }
         if (d_dir) {
-            // extras: (dir' - view')[3], <dir', view'>  with dir' = Rw2c * dir  ->  d dir = Rw2c^T (g[3:6] + g[6] * view')
-            const float3 ov = view_in_points(p.o, ray_dir(p.q, cand_ray(p.q, p.q.valid_list[p.row_samp[row]])));
+            // extras: (dir' - view')[3], <dir', view'>  with dir' = M_p dir (the point's frame) and view' in the frame of the sample's
+            // slot-0 point  ->  d dir = M_p^T (g[3:6] + g[6] * view')
+            const uint32_t s = p.q.valid_list[p.row_samp[row]];
+            const float3 ov = view_in_points<PP>(p.pts, p.o, view_point<PP>(p.q, s), ray_dir(p.q, cand_ray(p.q, s)));
             float gx = ge[3] + ge[6] * ov.x, gy = ge[4] + ge[6] * ov.y, gz = ge[5] + ge[6] * ov.z;
             float ox, oy, oz;
-            rot3T(p.o.Rw2c, gx, gy, gz, ox, oy, oz);
+            rot3T(point_frame<PP>(p.pts, p.o, pi), gx, gy, gz, ox, oy, oz);
             atomicAdd(&d_dir[3 * pi], ox); atomicAdd(&d_dir[3 * pi + 1], oy); atomicAdd(&d_dir[3 * pi + 2], oz);
         }
         if (d_conf) atomicAdd(&d_conf[pi], dwc[row] * p.wn[row]);   // straight-through clamp (gradiant_clamp :722-724)
@@ -622,7 +626,9 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     GemmCtx cx{(flags & 2) != 0, (flags & PNB_BWD_FP32_GEMM) == 0, L.part, PART_FLOATS * sizeof(float), d_err, st, (flags & PNB_BWD_FP32_RECOMPUTE) != 0};
     PNB_REQUIRE(!cx.tc || d_err, PNB_ERR_INVALID, "pnb_shade_backward: the tensor-core path needs d_err");
     // ---------------- forward recompute ----------------
-    k_bwd_build<<<wb, 256, 0, st>>>(p);
+    const bool pp = pts->rw2c != nullptr;                    // per-point frames
+    if (pp) k_bwd_build<true><<<wb, 256, 0, st>>>(p);
+    else k_bwd_build<false><<<wb, 256, 0, st>>>(p);
     gemm_nn(cx, L.X1, 288, mlp->w[0], 256, L.H1, 256, P, 256, 288, mlp->b[0], 1);
     gemm_nn(cx, L.H1, 256, mlp->w[1], 256, L.X3, 272, P, 256, 256, mlp->b[1], 1);   // H2 into X3[:, :256]
     gemm_nn(cx, L.X3, 272, mlp->w[2], 256, L.H3, 256, P, 256, 272, mlp->b[2], 1);
@@ -668,7 +674,8 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     colsum(L.G3, 256, P, 256, d_mlp_b[0], st);
     gemm_nt(cx, L.G3, 256, mlp->w[0], 256, L.G1, 288, P, 224, 256);                   // dX1: only the 224 feature columns are consumed (k_bwd_scatter; no xyz gradient)
     // scatter to the points
-    k_bwd_scatter<<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
+    if (pp) k_bwd_scatter<true><<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
+    else k_bwd_scatter<false><<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }

@@ -2,6 +2,8 @@
 // (k_shade_fwd), the tensor-core builders (k_shade_wg), the backward's recompute (k_bwd_build), and the kernels that need one
 // piece (k_color_wg, k_aux_outputs, k_composite, k_composite_bwd, k_bwd_scatter, k_bwd_reduce_fwd).
 //   sample position          diff_ray_marching.py:386
+//   point frames (Rw2c)      neural_points.py:717, point_aggregators.py:491-496 (uniform [3,3], or per point [N,3,3]: the pair's point
+//                            for dists and dir, the sample's slot-0 point for the view direction, :506, :526, :566)
 //   dists / linear weights   point_aggregators.py:727-814, :421-429 (conf_coefficient: neural_points.py:706-717, :722-724)
 //   block3 extras            point_aggregators.py:560-571
 //   raw2out_density / _color point_aggregators.py:262-273
@@ -66,10 +68,27 @@ __device__ __forceinline__ CandSample cand_sample(const pnb_query_t& q, uint32_t
     c.pos = ray_pos(q, c.dir, t);
     return c;
 }
-// the view direction in the points' canonical frame (:526)
-__device__ __forceinline__ float3 view_in_points(const pnb_shade_opts_t& o, float3 dir) {
+// ------------------------------------------------------------------------------------------ point frames
+// World -> canonical rotation of point pi, row-major (neural_points.Rw2c, gathered per neighbour: neural_points.py:717).  PP (per-point
+// frames, a compile-time parameter of every kernel that reads a frame): row pi of pts.rw2c [N][9], read in place; otherwise the one
+// uniform opts.Rw2c, and pi is not read.
+template <bool PP>
+__device__ __forceinline__ const float* point_frame(const pnb_points_t& pts, const pnb_shade_opts_t& o, int pi) {
+    if (PP) return pts.rw2c + (size_t)pi * 9;
+    return o.Rw2c;
+}
+// The point whose frame a sample's view direction is rotated into: its slot-0 neighbour (sampled_Rw2c[:,:,:,0], :495).  A sample
+// with a neighbour always has one in slot 0; an empty slot 0 (padding) reads point 0, as the reference's clamped gather.  Uniform
+// frames: no read.
+template <bool PP>
+__device__ __forceinline__ int view_point(const pnb_query_t& q, uint32_t s) {
+    return PP ? max(q.cand_pidx[(size_t)s * q.K], 0) : 0;
+}
+// the view direction in the frame of point p0 (the sample's view_point) (:506)
+template <bool PP>
+__device__ __forceinline__ float3 view_in_points(const pnb_points_t& pts, const pnb_shade_opts_t& o, int p0, float3 dir) {
     float3 v;
-    rot3(o.Rw2c, dir.x, dir.y, dir.z, v.x, v.y, v.z);
+    rot3(point_frame<PP>(pts, o, p0), dir.x, dir.y, dir.z, v.x, v.y, v.z);
     return v;
 }
 
@@ -89,8 +108,9 @@ struct PairGeom {
     int pi;          // point index (0 for an empty slot)
     float w;         // inverse-distance weight, not normalised
     float cc;        // conf_coefficient
-    float dist[6];   // world offset + perspective terms (:782-784), rotated into the points' frame
+    float dist[6];   // world offset + perspective terms (:782-784); the offset rotated into the point's frame
 };
+template <bool PP>
 __device__ __forceinline__ PairGeom pair_geom(const pnb_points_t& pts, const pnb_shade_opts_t& o, int pidx, float3 l) {
     PairGeom g;
     g.valid = pidx >= 0;
@@ -105,13 +125,15 @@ __device__ __forceinline__ PairGeom pair_geom(const pnb_points_t& pts, const pnb
     g.dist[5] = zpp - zsp;
     g.w = g.valid ? inv_dist_weight(dx, dy, dz) : 0.f;
     g.cc = conf_coef(__ldg(&pts.conf[g.pi]));
-    rot3(o.Rw2c, dx, dy, dz, g.dist[0], g.dist[1], g.dist[2]);
+    rot3(point_frame<PP>(pts, o, g.pi), dx, dy, dz, g.dist[0], g.dist[1], g.dist[2]);
     return g;
 }
-// block3 extras of point pi seen along the view direction ov (points' frame): colour (3), dir - view (3), <dir, view> (1)
+// block3 extras of point pi seen along the view direction ov (the sample's view frame): colour (3), dir - view (3), <dir, view> (1);
+// dir is rotated into the point's own frame (:566)
+template <bool PP>
 __device__ __forceinline__ void point_extras(const pnb_points_t& pts, const pnb_shade_opts_t& o, int pi, float3 ov, float* ex) {
     float ddx, ddy, ddz;
-    rot3(o.Rw2c, __ldg(&pts.dir[3 * pi]), __ldg(&pts.dir[3 * pi + 1]), __ldg(&pts.dir[3 * pi + 2]), ddx, ddy, ddz);
+    rot3(point_frame<PP>(pts, o, pi), __ldg(&pts.dir[3 * pi]), __ldg(&pts.dir[3 * pi + 1]), __ldg(&pts.dir[3 * pi + 2]), ddx, ddy, ddz);
     ex[0] = __ldg(&pts.color[3 * pi]); ex[1] = __ldg(&pts.color[3 * pi + 1]); ex[2] = __ldg(&pts.color[3 * pi + 2]);
     ex[3] = ddx - ov.x; ex[4] = ddy - ov.y; ex[5] = ddz - ov.z;
     ex[6] = ddx * ov.x + ddy * ov.y + ddz * ov.z;
@@ -165,19 +187,22 @@ struct Fp32Pair {
     int pidx;
     float wn;     // normalised weight
     float wc;     // weight * conf_coefficient (0 for an empty slot)
-    float3 ov;    // view direction in the points' frame
+    float3 ov;    // view direction in the sample's view frame
 };
+template <bool PP>
 __device__ __forceinline__ Fp32Pair fp32_pair(const pnb_query_t& q, const pnb_points_t& pts, const pnb_shade_opts_t& o, bool have,
                                               uint32_t s, int nk, int lane, float* vpe) {
     const int k = lane >> 2, part = lane & 3;   // neighbour slot, quarter of the feature vector
     CandSample cs = {};
     Fp32Pair r;
     r.pidx = -1;
+    int p0 = 0;
     if (have) {
         cs = cand_sample(q, s);
         if (k < nk) r.pidx = q.cand_pidx[(size_t)s * q.K + k];
+        p0 = view_point<PP>(q, s);
     }
-    r.ov = view_in_points(o, cs.dir);
+    r.ov = view_in_points<PP>(pts, o, p0, cs.dir);
     if (lane < 12) {
         const int dd = lane >> 2, jj = lane & 3;
         float sn, cn;
@@ -185,13 +210,14 @@ __device__ __forceinline__ Fp32Pair fp32_pair(const pnb_query_t& q, const pnb_po
         vpe[lane] = sn;
         vpe[12 + lane] = cn;
     }
-    r.g = pair_geom(pts, o, r.pidx, cs.pos);
+    r.g = pair_geom<PP>(pts, o, r.pidx, cs.pos);
     float wsum = part == 0 ? r.g.w : 0.f;       // sum over the 8 slots
     for (int d = 16; d > 0; d >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, d);
     r.wn = norm_weight(r.g.w, wsum);
     r.wc = r.g.valid ? r.wn * r.g.cc : 0.f;
     return r;
 }
+template <bool PP>
 __device__ __forceinline__ void fp32_pair_row(const pnb_points_t& pts, const pnb_shade_opts_t& o, const Fp32Pair& r, int lane, float* xr,
                                               float* ex) {
     const int part = lane & 3;
@@ -222,7 +248,7 @@ __device__ __forceinline__ void fp32_pair_row(const pnb_points_t& pts, const pnb
         xr[224 + i * 2 + 1] = cn;
     }
     if (part == 0) { xr[284] = 0.f; xr[285] = 0.f; xr[286] = 0.f; xr[287] = 0.f; }
-    if (part == 1) point_extras(pts, o, g.pi, r.ov, ex);
+    if (part == 1) point_extras<PP>(pts, o, g.pi, r.ov, ex);
 }
 
 }  // namespace pnb

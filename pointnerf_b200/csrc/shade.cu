@@ -152,6 +152,8 @@ __device__ __forceinline__ void dense8(const float* __restrict__ in, int sin_, f
     __syncthreads();
 }
 
+// PP: per-point frames (pts.rw2c != NULL), a compile-time parameter
+template <bool PP>
 __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     ShadeSmem& sm = *reinterpret_cast<ShadeSmem*>(smem_raw);
@@ -170,11 +172,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
             const uint32_t s = have ? q.valid_list[vi] : 0xffffffffu;
             float* xr = &sm.X[row * XS];
             if (lane == 0) sm.samp[warp] = s;
-            const Fp32Pair pr = fp32_pair(q, p.pts, p.o, have, s, q.K, lane, &sm.view[warp][3]);
+            const Fp32Pair pr = fp32_pair<PP>(q, p.pts, p.o, have, s, q.K, lane, &sm.view[warp][3]);
             if (lane < 3) sm.view[warp][lane] = lane == 0 ? pr.ov.x : lane == 1 ? pr.ov.y : pr.ov.z;
             if (part == 0) sm.wc[row] = pr.wc;
             if (pr.g.valid) {
-                fp32_pair_row(p.pts, p.o, pr, lane, xr, sm.E[row]);
+                fp32_pair_row<PP>(p.pts, p.o, pr, lane, xr, sm.E[row]);
             } else {
                 for (int c = part; c < 288; c += 4) xr[c] = 0.f;
                 if (part == 1)
@@ -406,14 +408,16 @@ extern "C" int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, 
     PNB_CHECK_CUDA(cudaGetDevice(&dev));
     PNB_REQUIRE(dev >= 0 && dev < 64, PNB_ERR_UNSUPPORTED, "pnb_shade_forward: device ordinal %d", dev);
     if (!smem_set[dev]) {
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
         PNB_CHECK_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
         smem_set[dev] = 1;
     }
     const int n_sm = n_sm_of[dev];
     ShadeParams p;
     p.q = *q; p.pts = *pts; p.mlp = *mlp; p.o = *opts; p.sigma_rgb = (float4*)d_sigma_rgb;
-    k_shade_fwd<<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
+    if (pts->rw2c) k_shade_fwd<true><<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
+    else k_shade_fwd<false><<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }

@@ -101,7 +101,8 @@ __device__ __forceinline__ float seg_sum8(float v, int lane, int st, int cnt) {
 //   part 1 = operand columns 152..287 (PE of features 20..31, PE of the 6 distances), extras operand, weight*conf
 // FROZEN (part 1 only, one builder thread per row): the feature columns come from the per-point table, so the row is part 1
 // without the feature PE and with the distance PE at operand columns 0..63 (K blocks 0, 1); it also records the row's point.
-template <int PART, bool FROZEN, class SmemT>
+// PP: per-point frames (pair_inputs.cuh, point_frame).
+template <int PART, bool FROZEN, bool PP, class SmemT>
 __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& p, int row, int n_valid, int pvi, int pk, int pst, int pcnt) {
     using namespace tc;
     static_assert(PART == 0 || PART == 1, "two parts per row");
@@ -111,11 +112,11 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
     constexpr int DCOL = FROZEN ? 0 : 224;                              // first operand column of the distance PE
     constexpr int C_LO = P1 && !FROZEN ? 19 : 0, C_HI = P0 ? 19 : FROZEN ? 8 : 36;   // 16-byte chunks (column / 8) of this part
     const pnb_query_t& q = p.q;
-    int pidx = -1;
+    int pidx = -1, p0 = 0;
     CandSample cs = {};
     if (pvi >= 0 && pvi < n_valid) {
         const uint32_t s = q.valid_list[pvi];
-        if (P1) cs = cand_sample(q, s);
+        if (P1) { cs = cand_sample(q, s); p0 = view_point<PP>(q, s); }
         if (pk < q.K) pidx = q.cand_pidx[(size_t)s * q.K + pk];
     }
     if (FROZEN) sm.prow[row] = pidx;
@@ -124,8 +125,8 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
     PairGeom g;
     float3 ov;
     if (P1) {
-        ov = view_in_points(p.o, cs.dir);
-        g = pair_geom(p.pts, p.o, pidx, cs.pos);
+        ov = view_in_points<PP>(p.pts, p.o, p0, cs.dir);
+        g = pair_geom<PP>(p.pts, p.o, pidx, cs.pos);
         const float wsum = seg_sum8(g.w, row & 31, pst, pcnt);   // every lane takes part in the shuffles
         sm.wc[row] = valid ? norm_weight(g.w, wsum) * g.cc : 0.f;
     }
@@ -158,7 +159,7 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
             dp[60] = dp[61] = dp[62] = dp[63] = 0.f;
 #pragma unroll
             for (int c = 0; c < 8; ++c) store_chunk8_a1(sm, row, (DCOL + 8 * c) >> 5, (DCOL + 8 * c) & 31, dp + 8 * c);
-            point_extras(p.pts, p.o, pi, ov, ex);
+            point_extras<PP>(p.pts, p.o, pi, ov, ex);
         }
     } else {
         float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -485,8 +486,9 @@ __device__ __forceinline__ uint32_t step_image(uint32_t j, bool frozen) {
 }
 }  // namespace hw
 
-// O1: agg_intrp_order == 1 as a compile-time flag (the alpha dot product over the K-aggregated feature)
-template <bool FROZEN, bool O1>
+// O1: agg_intrp_order == 1 as a compile-time flag (the alpha dot product over the K-aggregated feature); PP: per-point frames
+// (pts.rw2c != NULL), compile-time as well, so that the uniform-frame builds keep their registers
+template <bool FROZEN, bool O1, bool PP>
 __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -538,9 +540,9 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
                 const int cj = __shfl_sync(0xffffffffu, c, qr.j);
                 if (lane == 0 && part == 0) { sm.qhead[qw] = head; sm.qfirst[qw] = first; sm.qtotal[qw] = (uint32_t)total; }
                 const int pvi = qr.live ? (int)p.vorder[first + qr.j] : -1;
-                if (FROZEN) build_pair_part<1, true>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else if (part == 0) build_pair_part<0, false>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else build_pair_part<1, false>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                if (FROZEN) build_pair_part<1, true, PP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else if (part == 0) build_pair_part<0, false, PP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else build_pair_part<1, false, PP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
             }
             fence_proxy_async();
             named_bar_sync(1, hw::NTHR);
@@ -664,6 +666,7 @@ struct ColorTcParams {
     int hbar_cap;
     float4* sigma_rgb;
     int* err;
+    pnb_points_t pts;               // PP: the per-point frames of the view direction
 };
 
 // =====================================================================================================================
@@ -685,6 +688,8 @@ struct Smem {
 };
 }  // namespace hcw
 
+// PP: per-point frames (the view direction in the frame of each sample's slot-0 point)
+template <bool PP>
 __global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
     using namespace hcw;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -726,7 +731,7 @@ __global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
             for (int i = 0; i < 32; ++i) pe[i] = 0.f;
             if (vi < n_valid) {
                 const uint32_t s = q.valid_list[vi];
-                const float3 v = view_in_points(p.o, ray_dir(q, cand_ray(q, s)));
+                const float3 v = view_in_points<PP>(p.pts, p.o, view_point<PP>(q, s), ray_dir(q, cand_ray(q, s)));
                 const float ov[3] = {v.x, v.y, v.z};
 #pragma unroll
                 for (int d = 0; d < 3; ++d) {     // ori=True layout: sin block (d*4+j) then cos block
@@ -929,11 +934,13 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
     static_assert(sizeof(hw::Smem) + 128 <= kSmemMax, "pair kernel shared-memory carve-out exceeds the per-block limit");
     static_assert(sizeof(hcw::Smem) + 128 <= kSmemMax, "colour kernel shared-memory carve-out exceeds the per-block limit");
     if (!configured[dev]) {
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_wg<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_wg<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_wg<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_wg<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
+        const void* pair_kernels[8] = {(const void*)k_shade_wg<false, false, false>, (const void*)k_shade_wg<false, true, false>,
+                                       (const void*)k_shade_wg<true, false, false>, (const void*)k_shade_wg<true, true, false>,
+                                       (const void*)k_shade_wg<false, false, true>, (const void*)k_shade_wg<false, true, true>,
+                                       (const void*)k_shade_wg<true, false, true>, (const void*)k_shade_wg<true, true, true>};
+        for (const void* k : pair_kernels) PNB_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
         PNB_CHECK_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
         configured[dev] = 1;
     }
@@ -953,14 +960,14 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
         k_pack_quads<<<(n_sc + 7) / 8, 256, 0, stream>>>(p.q, cap, w.sc_quads, w.quad_local, w.vorder, w.vcntp, (float4*)d_sigma_rgb);
         k_pack_scan<<<1, 1024, 0, stream>>>(p.q, cap, w.sc_quads, w.quad_first, w.pack_cnt);
         k_pack_place<<<(cap + 255) / 256, 256, 0, stream>>>(p.q, cap, w.sc_quads, w.quad_local, w.quad_first);
-        const bool o1 = opts->agg_intrp_order == 1;              // a compile-time flag of the kernel
-        if (frozen) {
-            if (o1) k_shade_wg<true, true><<<n_cta, hw::NTHR, smem_pair, stream>>>(p);
-            else k_shade_wg<true, false><<<n_cta, hw::NTHR, smem_pair, stream>>>(p);
-        } else {
-            if (o1) k_shade_wg<false, true><<<n_cta, hw::NTHR, smem_pair, stream>>>(p);
-            else k_shade_wg<false, false><<<n_cta, hw::NTHR, smem_pair, stream>>>(p);
-        }
+        const bool o1 = opts->agg_intrp_order == 1;              // compile-time flags of the kernel
+        const bool pp = pts->rw2c != nullptr;
+        void (*kern)(ShadeTcParams) =
+            frozen ? (o1 ? (pp ? k_shade_wg<true, true, true> : k_shade_wg<true, true, false>)
+                         : (pp ? k_shade_wg<true, false, true> : k_shade_wg<true, false, false>))
+                   : (o1 ? (pp ? k_shade_wg<false, true, true> : k_shade_wg<false, true, false>)
+                         : (pp ? k_shade_wg<false, false, true> : k_shade_wg<false, false, false>));
+        kern<<<n_cta, hw::NTHR, smem_pair, stream>>>(p);
     }
     if (flags & PNB_TC_COLOR) {
         ColorTcParams ct;
@@ -968,7 +975,9 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
         for (int i = 0; i < 3; ++i) ct.bias[i] = mlp->b[5 + i];
         ct.w3t = mlp->w[8]; ct.b3 = mlp->b[8];
         ct.hbar = w.hbar; ct.sigma = w.sigma; ct.hbar_cap = max_valid_samples; ct.sigma_rgb = (float4*)d_sigma_rgb; ct.err = d_err;
-        k_color_wg<<<n_cta, hcw::NTHR, smem_color, stream>>>(ct);
+        ct.pts = *pts;
+        if (pts->rw2c) k_color_wg<true><<<n_cta, hcw::NTHR, smem_color, stream>>>(ct);
+        else k_color_wg<false><<<n_cta, hcw::NTHR, smem_color, stream>>>(ct);
     }
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;

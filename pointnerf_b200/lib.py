@@ -48,7 +48,7 @@ class Mlp(C.Structure):
 
 class Points(C.Structure):
     _fields_ = [("xyz", C.c_void_p), ("emb", C.c_void_p), ("color", C.c_void_p), ("dir", C.c_void_p),
-                ("conf", C.c_void_p), ("N", C.c_int32)]
+                ("conf", C.c_void_p), ("N", C.c_int32), ("rw2c", C.c_void_p)]
 
 
 GC = dict(n_occ=0, max_pts=1, overflow_o=2, overflow_p=3, n_inrange=4, slot0_cell=5, first_pt=6)

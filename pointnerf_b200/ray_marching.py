@@ -140,10 +140,17 @@ class MlpPack:
         return self.desc
 
 
+def per_point_rw2c(npnts):
+    """True when the module carries one world->canonical rotation per point (Rw2c [N,3,3], edited / composed scenes)."""
+    return npnts.Rw2c is not None and npnts.Rw2c.dim() == 3
+
+
 def points_desc_of(npnts):
-    """pnb_points_t over the parameter tensors of a NeuralPoints-like module (ours or the reference's)."""
-    if npnts.Rw2c is not None and npnts.Rw2c.dim() != 2:
-        raise NotImplementedError("pnb200: per-point Rw2c is not part of the implemented hot path")
+    """pnb_points_t over the parameter tensors of a NeuralPoints-like module (ours or the reference's).  A per-point Rw2c [N,3,3] is
+    read in place by the kernels (pnb_points_t.rw2c); a uniform [3,3] one goes by value in the shading options (rw2c_host_of)."""
+    R = npnts.Rw2c
+    if R is not None and R.dim() not in (2, 3):
+        raise _lib.PnbError("pnb200: neural_points.Rw2c must be [3,3] or [N,3,3], got %s" % (tuple(R.shape),))
     for name in ("points_embeding", "points_color", "points_dir", "points_conf"):
         if getattr(npnts, name, None) is None:
             raise NotImplementedError("pnb200: neural_points.%s is None; the hot path needs point_{conf,dir,color}_mode=1" % name)
@@ -156,6 +163,12 @@ def points_desc_of(npnts):
         raise NotImplementedError("pnb200: point_features_dim must be 32")
     p.xyz, p.emb, p.color, p.dir, p.conf = (t.data_ptr() for t in tens)
     p.N = npnts.xyz.shape[0]
+    if per_point_rw2c(npnts):
+        if tuple(R.shape) != (p.N, 3, 3) or R.dtype != torch.float32 or not R.is_contiguous() or R.device != npnts.xyz.device:
+            raise _lib.PnbError("pnb200: a per-point neural_points.Rw2c must be a contiguous fp32 [N,3,3] tensor on the points' device "
+                                "(N=%d), got %s %s on %s%s" % (p.N, tuple(R.shape), R.dtype, R.device,
+                                                               "" if R.is_contiguous() else ", not contiguous"))
+        p.rw2c = R.data_ptr()
     return p
 
 
@@ -185,6 +198,7 @@ class NeuralPoints(nn.Module):
 
     def set_points(self, points_xyz, points_embeding, points_color=None, points_dir=None, points_conf=None,
                    parameter=True, Rw2c=None, **_):
+        """neural_points.py:400-467.  Rw2c: None (identity), one [3,3] rotation for the whole cloud, or one per point [N,3,3]."""
         mk = (lambda t, g: nn.Parameter(t.contiguous(), requires_grad=g)) if parameter else (lambda t, g: t.contiguous())
         o = self.opt
         self.xyz = mk(points_xyz, getattr(o, "xyz_grad", 0) > 0)
@@ -197,6 +211,25 @@ class NeuralPoints(nn.Module):
         # a supplied Rw2c is part of the state dict, as in the reference (neural_points.py:463-467); the default stays a plain eye(3)
         self.Rw2c = torch.eye(3, device=points_xyz.device) if Rw2c is None else \
             nn.Parameter(Rw2c.to(points_xyz.device).float().contiguous(), requires_grad=False)
+        self.querier.clean_up()
+
+    def editing_set_points(self, points_xyz, points_embeding, points_color=None, points_dir=None, points_conf=None,
+                           parameter=False, Rw2c=None, eulers=None):
+        """models/neural_points/neural_points.py:470-484 (run/editing.py): install the point cloud of an edited or
+        composed scene as plain tensors (no parameters), with opt.default_conf in (0, 1] overriding every conf.  Rw2c: None
+        (identity), [3,3] or one rotation per point [N,3,3]."""
+        dc = float(getattr(self.opt, "default_conf", -1.0))
+        if 0.0 < dc <= 1.0 and points_conf is not None:
+            points_conf = torch.ones_like(points_conf) * dc
+        for name in ("xyz", "points_embeding", "points_conf", "points_dir", "points_color", "Rw2c"):
+            if name in self._parameters:
+                del self._parameters[name]
+        self.xyz = points_xyz
+        self.points_embeding = points_embeding
+        self.points_dir = points_dir
+        self.points_conf = points_conf
+        self.points_color = points_color
+        self.Rw2c = torch.eye(3, device=points_xyz.device, dtype=points_xyz.dtype) if Rw2c is None else Rw2c
         self.querier.clean_up()
 
     def reset_querier(self):
@@ -218,17 +251,29 @@ class NeuralPoints(nn.Module):
         self.points_conf = self._wrap(self.points_conf[:, mask, :], getattr(o, "conf_grad", 1) > 0)
         self.points_dir = self._wrap(self.points_dir[:, mask, :], getattr(o, "dir_grad", 1) > 0)
         self.points_color = self._wrap(self.points_color[:, mask, :], getattr(o, "color_grad", 1) > 0)
+        if per_point_rw2c(self):                                  # :367-369
+            self.Rw2c = self._wrap(self.Rw2c[mask], False)
         self.querier.clean_up()
         return int((~mask).sum())
 
     def grow_points(self, add_xyz, add_embedding, add_color, add_dir, add_conf, add_eulers=None, add_Rw2c=None):
-        """/root/reference/models/neural_points/neural_points.py:373-399: append points (new parameters)."""
+        """/root/reference/models/neural_points/neural_points.py:373-399: append points (new parameters).  A per-point Rw2c [N,3,3]
+        grows by add_Rw2c [M,3,3] along the point dimension (the reference's torch.cat(..., dim=1) of :397-398 cannot run on that
+        shape; DESIGN.md section 5); without add_Rw2c the new points would have no frame, which raises ValueError."""
         o = self.opt
+        pp = per_point_rw2c(self)
+        if pp and add_Rw2c is None:
+            raise ValueError("pnb200: growing a point cloud with per-point Rw2c [N,3,3] needs add_Rw2c [M,3,3] for the new points")
+        if pp and tuple(add_Rw2c.shape) != (add_xyz.shape[0], 3, 3):
+            raise ValueError("pnb200: add_Rw2c has shape %s, the %d new points need [%d,3,3]"
+                             % (tuple(add_Rw2c.shape), add_xyz.shape[0], add_xyz.shape[0]))
         self.xyz = self._wrap(torch.cat([self.xyz, add_xyz], dim=0), getattr(o, "xyz_grad", 0) > 0)
         self.points_embeding = self._wrap(torch.cat([self.points_embeding, add_embedding[None, ...]], dim=1), getattr(o, "feat_grad", 1) > 0)
         self.points_conf = self._wrap(torch.cat([self.points_conf, add_conf[None, ...]], dim=1), getattr(o, "conf_grad", 1) > 0)
         self.points_dir = self._wrap(torch.cat([self.points_dir, add_dir[None, ...]], dim=1), getattr(o, "dir_grad", 1) > 0)
         self.points_color = self._wrap(torch.cat([self.points_color, add_color[None, ...]], dim=1), getattr(o, "color_grad", 1) > 0)
+        if pp:
+            self.Rw2c = self._wrap(torch.cat([self.Rw2c, add_Rw2c.to(self.Rw2c.device, self.Rw2c.dtype)], dim=0), False)
         self.querier.clean_up()
 
     def points_desc(self):
@@ -447,7 +492,8 @@ class NeuralPointsRayMarching(nn.Module):
         # cost one small D2H copy (the reference does the same with near/far/intrinsic, neural_points.py:704)
         cp, rt, bg = _to_list(campos)[:3], _to_list(camrotc2w)[:9], _to_list(bg_color)[:3]
         q = npnts.querier.run_query(npnts.xyz.detach(), raydir, cp, float(near), float(far), t=t, want_counters=want_counters)
-        o = make_cam_opts(cp, rt, Rw2c=rw2c_host_of(npnts),
+        # per-point frames go to the kernels through pnb_points_t.rw2c (read in place); the uniform slot of the options is unused then
+        o = make_cam_opts(cp, rt, Rw2c=None if per_point_rw2c(npnts) else rw2c_host_of(npnts),
                           vsize_z=float(opt.vsize[2]), bg_color=bg, raydist_mode_unit=int(getattr(opt, "raydist_mode_unit", 0)),
                           agg_intrp_order=int(getattr(opt, "agg_intrp_order", 2)))
         cap = q.desc.cap_samples

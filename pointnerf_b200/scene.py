@@ -88,6 +88,19 @@ def make_points(cfg: SceneConfig, device="cpu"):
     return {k: v.to(device) for k, v in out.items()}
 
 
+def edit_frames(xyz, seed=11):
+    """Per-point Rw2c [N,3,3] shaped like a scene edit (the reference's run/editing.py:186-212 stores the rotation of each object's
+    rigid transform on its points): the cloud split by sign(x) into two objects, rotated by seeded angles in [0.4, 1.2) rad about z
+    (x < 0) and about x (x >= 0).  Samples near the seam x = 0 have neighbours in both frames."""
+    g = torch.Generator().manual_seed(seed)
+    a, b = (0.4 + 0.8 * torch.rand(2, generator=g)).tolist()
+    ca, sa, cb, sb = math.cos(a), math.sin(a), math.cos(b), math.sin(b)
+    Rz = torch.tensor([[ca, -sa, 0.0], [sa, ca, 0.0], [0.0, 0.0, 1.0]], dtype=torch.float32)
+    Rx = torch.tensor([[1.0, 0.0, 0.0], [0.0, cb, -sb], [0.0, sb, cb]], dtype=torch.float32)
+    left = (xyz[:, 0] < 0)[:, None, None]
+    return torch.where(left, Rz.to(xyz.device), Rx.to(xyz.device)).contiguous()
+
+
 def make_intrinsic(cfg: SceneConfig):
     f = 0.5 * cfg.W / math.tan(0.5 * cfg.fov_x)
     return np.array([[f, 0, cfg.W / 2], [0, f, cfg.H / 2], [0, 0, 1]], dtype=np.float32)
