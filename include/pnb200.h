@@ -226,8 +226,10 @@ int pnb_shade_tc_tables(void* ws, size_t ws_bytes, int max_valid_samples, void**
 
 /* ---- backward (per-scene optimisation batches) ----
  * Replaces loss.backward() through the reference's eager autograd graph
- * (models/mvs_points_volumetric_model.py:98-118): given d(loss)/d(ray_color) [R,3] (full-R layout of
- * pnb_composite_forward) accumulates gradients of points_embeding [N,32], points_color [N,3], points_dir [N,3],
+ * (models/mvs_points_volumetric_model.py:98-118): given d(loss)/d(ray_color) [R,3], d(loss)/d(opacity) [R,SR] and
+ * d(loss)/d(bg_T) [R] (the full-R layout of pnb_composite_forward; each may be NULL, at least one is given; NULL means that output
+ * is not in the loss, and with d_ray_color alone the call is the colour-only backward) accumulates gradients of
+ * points_embeding [N,32], points_color [N,3], points_dir [N,3],
  * points_conf [N] (any may be NULL) and of the 9 MLP layers in the layout of pnb_mlp_t (W^T [K_pad][N] and bias; the
  * caller zero-initialises all accumulators).  d_sigma_rgb_fwd: the forward's per-candidate (sigma, rgb) buffer.
  * n_valid / n_pairs: host copies of counters[PNB_QC_N_VALID] / [PNB_QC_N_PAIRS] (the pair-level buffers hold one row per valid pair).  ws >= pnb_backward_bytes.  The activations are recomputed and every layer
@@ -241,8 +243,9 @@ enum {
 };
 size_t pnb_backward_bytes(int n_valid, int cap_samples);
 int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts, const pnb_mlp_t* mlp, const pnb_shade_opts_t* opts,
-                       const float* d_sigma_rgb_fwd, const float* d_ray_color, int n_valid, int n_pairs, float* d_emb, float* d_color,
-                       float* d_dir, float* d_conf, float* const* d_mlp_w, float* const* d_mlp_b, void* ws,
+                       const float* d_sigma_rgb_fwd, const float* d_ray_color /* [R,3] or NULL */,
+                       const float* d_opacity /* [R,SR] or NULL */, const float* d_bg_T /* [R] or NULL */, int n_valid, int n_pairs,
+                       float* d_emb, float* d_color, float* d_dir, float* d_conf, float* const* d_mlp_w, float* const* d_mlp_b, void* ws,
                        size_t ws_bytes, int flags, int* d_err, pnb_stream_t stream);
 
 #ifdef __cplusplus

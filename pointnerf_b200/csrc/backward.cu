@@ -4,7 +4,9 @@
 //   ray_march        /root/reference/models/rendering/diff_ray_marching.py:508-554
 //   viewmlp          /root/reference/models/aggregators/point_aggregators.py:488-644
 //   index_select     /root/reference/models/neural_points/neural_points.py:706-717 (backward = index_add into [1,N,.])
-// Gradients produced: points_embeding [N,32], points_color [N,3], points_dir [N,3], points_conf [N] (through
+// Gradients consumed: d loss / d ray_color [R,3], d loss / d opacity [R,SR] and d loss / d bg_T [R] (the outputs ray_march keeps in the
+// autograd graph, returned as coarse_raycolor / coarse_point_opacity / coarse_is_background, neural_points_volumetric_model.py:312-324),
+// each optional.  Gradients produced: points_embeding [N,32], points_color [N,3], points_dir [N,3], points_conf [N] (through
 // weight*conf_coefficient, straight-through clamp :722-724), and the 18 MLP tensors (in the W^T layout of pnb_mlp_t).
 // xyz receives no gradient (xyz_grad = 0 in every shipped script).
 //
@@ -502,15 +504,21 @@ __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* _
     }
 }
 
-// Composite backward: per ray, d ray_color -> d(sigma, rgb) of each of its candidate samples.
+// Composite backward: per ray, d ray_color, d opacity and d bg_T -> d(sigma, rgb) of each of its candidate samples.
 struct CompBwdParams {
     pnb_query_t q;
     pnb_shade_opts_t o;
     const float4* sigma_rgb;
-    const float* d_ray_color;   // [R,3]
+    const float* d_ray_color;   // [R,3]; NULL (EXT only): no colour term
     float4* d_sigma_rgb;        // [cap]
+    const float* d_opacity;     // [R,SR] or NULL (EXT only)
+    const float* d_bg_T;        // [R] or NULL (EXT only)
 };
 
+// EXT: the upstream gradients of opacity and bg_T (each optional, as is the colour's); without it the kernel reads d ray_color only.
+// With T_{j+1} = T_j (1 - o_j + 1e-10) and bg_T = T_end, the bg_T gradient enters the suffix beside g.bg, and the opacity gradient
+// adds to d o_j directly.
+template <bool EXT>
 __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
     int r = blockIdx.x * blockDim.x + threadIdx.x;
     const pnb_query_t& q = p.q;
@@ -523,7 +531,10 @@ __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
         return;
     }
     const float3 dir = ray_dir(q, r);
-    const float gR = p.d_ray_color[3 * r], gG = p.d_ray_color[3 * r + 1], gB = p.d_ray_color[3 * r + 2];
+    const bool col = !EXT || p.d_ray_color;
+    const float gR = col ? p.d_ray_color[3 * r] : 0.f, gG = col ? p.d_ray_color[3 * r + 1] : 0.f,
+                gB = col ? p.d_ray_color[3 * r + 2] : 0.f;
+    const float* g_o = EXT && p.d_opacity ? p.d_opacity + (size_t)r * q.SR : nullptr;
     // pass 1 (front to back): opacity, ray distance and transmittance of every candidate (local arrays, SR <= 128)
     float o_[PNB_MAX_SR], rd_[PNB_MAX_SR], T_[PNB_MAX_SR];
     float Tend;
@@ -538,8 +549,10 @@ __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
         }
         Tend = T;
     }
-    // pass 2 (back to front): suffix_j = g.bg T_end + sum_{i>j} g.rgb_i o_i T_i   (no cancellation)
-    float suffix = (gR * p.o.bg_color[0] + gG * p.o.bg_color[1] + gB * p.o.bg_color[2]) * Tend;
+    // pass 2 (back to front): suffix_j = (g.bg + g_T) T_end + sum_{i>j} g.rgb_i o_i T_i   (no cancellation)
+    float gbg = gR * p.o.bg_color[0] + gG * p.o.bg_color[1] + gB * p.o.bg_color[2];
+    if (EXT && p.d_bg_T) gbg += p.d_bg_T[r];
+    float suffix = gbg * Tend;
     for (int j = n - 1; j >= 0; --j) {
         float4 out = make_float4(0.f, 0.f, 0.f, 0.f);
         if (q.samp_nvalid[s0 + j] > 0) {
@@ -548,6 +561,7 @@ __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
             float gdot = gR * v.y + gG * v.z + gB * v.w;
             float bw = o1 * T;
             float d_o = gdot * T - suffix / (1.0f - o1 + 1e-10f);
+            if (EXT && g_o) d_o += g_o[j];               // added last: a zero g_o leaves the colour-only bits unchanged
             out.x = d_o * rd_[j] * (1.0f - o1);              // d o / d sigma = rd * exp(-sigma rd)
             out.y = gR * bw; out.z = gG * bw; out.w = gB * bw;
             suffix += gdot * bw;
@@ -595,21 +609,26 @@ extern "C" size_t pnb_backward_bytes(int n_valid, int cap_samples) { return carv
 
 // d_mlp_w[i] / d_mlp_b[i]: gradient accumulators in the layout of pnb_mlp_t (W^T [K_pad][N], bias [N]); the caller
 // zero-initialises them.  Point gradients are accumulated (atomicAdd) into d_emb/d_color/d_dir/d_conf (caller zeroes);
-// any of them may be NULL.  n_valid: host copy of counters[PNB_QC_N_VALID] of the query.
+// any of them may be NULL.  Upstream gradients: d_ray_color [R,3], d_opacity [R,SR], d_bg_T [R], each may be NULL (at least one is
+// given).  n_valid: host copy of counters[PNB_QC_N_VALID] of the query.
 extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts, const pnb_mlp_t* mlp,
                                   const pnb_shade_opts_t* opts, const float* d_sigma_rgb_fwd, const float* d_ray_color,
-                                  int n_valid, int n_pairs, float* d_emb, float* d_color, float* d_dir, float* d_conf,
-                                  float* const* d_mlp_w, float* const* d_mlp_b, void* ws, size_t ws_bytes, int flags, int* d_err,
-                                  pnb_stream_t stream_) {
+                                  const float* d_opacity, const float* d_bg_T, int n_valid, int n_pairs, float* d_emb, float* d_color,
+                                  float* d_dir, float* d_conf, float* const* d_mlp_w, float* const* d_mlp_b, void* ws, size_t ws_bytes,
+                                  int flags, int* d_err, pnb_stream_t stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    PNB_REQUIRE(q && pts && mlp && opts && d_sigma_rgb_fwd && d_ray_color && d_mlp_w && d_mlp_b && ws, PNB_ERR_INVALID,
+    PNB_REQUIRE(q && pts && mlp && opts && d_sigma_rgb_fwd && d_mlp_w && d_mlp_b && ws, PNB_ERR_INVALID,
                 "pnb_shade_backward: null argument");
+    PNB_REQUIRE(d_ray_color || d_opacity || d_bg_T, PNB_ERR_INVALID,
+                "pnb_shade_backward: no upstream gradient (d_ray_color, d_opacity and d_bg_T are all NULL)");
     Layout L = carve(ws, ws_bytes, n_valid, q->cap_samples);
     PNB_REQUIRE(L.bytes <= ws_bytes, PNB_ERR_WORKSPACE, "pnb_shade_backward: workspace %zu < required %zu", ws_bytes, L.bytes);
     // composite backward first (also covers n_valid == 0)
     CompBwdParams cp;
     cp.q = *q; cp.o = *opts; cp.sigma_rgb = (const float4*)d_sigma_rgb_fwd; cp.d_ray_color = d_ray_color; cp.d_sigma_rgb = L.d_sigma_rgb;
-    k_composite_bwd<<<(q->R + 127) / 128, 128, 0, st>>>(cp);
+    cp.d_opacity = d_opacity; cp.d_bg_T = d_bg_T;
+    if (d_ray_color && !d_opacity && !d_bg_T) k_composite_bwd<false><<<(q->R + 127) / 128, 128, 0, st>>>(cp);   // colour-only loss
+    else k_composite_bwd<true><<<(q->R + 127) / 128, 128, 0, st>>>(cp);
     if (n_valid <= 0) { PNB_CHECK_CUDA(cudaGetLastError()); return PNB_OK; }
     PNB_REQUIRE(n_pairs >= n_valid && n_pairs <= n_valid * PNB_MAX_K, PNB_ERR_INVALID, "pnb_shade_backward: n_pairs %d inconsistent with n_valid %d", n_pairs, n_valid);
     const int S = n_valid, P = n_pairs;      // pair-level buffers hold one row per VALID (sample, neighbour) pair

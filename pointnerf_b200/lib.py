@@ -136,7 +136,7 @@ def load():
     lib.pnb_backward_bytes.argtypes = [C.c_int, C.c_int]
     lib.pnb_shade_backward.restype = C.c_int
     lib.pnb_shade_backward.argtypes = [C.POINTER(Query), C.POINTER(Points), C.POINTER(Mlp), C.POINTER(ShadeOpts), C.c_void_p,
-                                       C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p]
     _lib = lib
     return lib

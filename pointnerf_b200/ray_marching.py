@@ -280,9 +280,22 @@ class NeuralPoints(nn.Module):
         return points_desc_of(self)
 
 
+def _upstream_grad(g, shape, name):
+    """An upstream gradient of _RenderFn as pnb_shade_backward reads it: None (the output is not in the loss) or contiguous fp32 of
+    the output's full-R shape."""
+    if g is None:
+        return None
+    if tuple(g.shape) != shape:
+        raise _lib.PnbError("pnb200: the gradient of %s has shape %s, expected %s" % (name, tuple(g.shape), shape))
+    return g.contiguous().float()
+
+
 class _RenderFn(torch.autograd.Function):
-    """Differentiable face of the fused path: ray_color[R,3] = f(points_embeding, points_color, points_dir,
-    points_conf, 18 MLP tensors).  Backward = pnb_shade_backward (activations recomputed, layer GEMMs on wgmma / BF16x3)."""
+    """Differentiable face of the fused path: ray_color[R,3], opacity[R,SR] and bg_T[R] = f(points_embeding, points_color,
+    points_dir, points_conf, 18 MLP tensors), all three in the autograd graph as in the reference (ray_march,
+    diff_ray_marching.py:508-554).  Backward = pnb_shade_backward (activations recomputed, layer GEMMs on wgmma / BF16x3).
+    Gradients are not materialised: an output outside the loss reaches the backward as None and goes to the kernel as NULL, so a
+    colour-only loss takes the colour-only composite backward."""
 
     @staticmethod
     def forward(ctx, mod, run_args, emb, color, pdir, conf, *mlp_params):
@@ -296,11 +309,16 @@ class _RenderFn(torch.autograd.Function):
         ctx.sigma_rgb = mod._sigma_rgb          # forward (sigma, rgb) per candidate; valid until the next _run
         ctx.needs = [t.requires_grad for t in (emb, color, pdir, conf)]
         ctx.mlp_shapes = [tuple(t.shape) for t in mlp_params]
-        ctx.mark_non_differentiable(opacity, bg_T, ray_mask)
+        ctx.shapes = (tuple(ray_color.shape), tuple(opacity.shape), tuple(bg_T.shape))
+        ctx.mark_non_differentiable(ray_mask)
+        ctx.set_materialize_grads(False)
         return ray_color, opacity, bg_T, ray_mask
 
     @staticmethod
     def backward(ctx, g_color, g_op, g_bg, g_mask):
+        if g_color is None and g_op is None and g_bg is None:
+            # reached through a consumer that returned no gradient for these outputs: nothing flows back
+            return (None,) * (6 + len(ctx.mlp_shapes))
         lib = _lib.load()
         mod, q = ctx.mod, ctx.q
         if mod._generation != ctx.generation:
@@ -308,8 +326,10 @@ class _RenderFn(torch.autograd.Function):
                                 "same module (two forwards before one backward, or an eval render in between); call backward() "
                                 "before the next forward")
         npnts = mod.neural_points
-        dev = g_color.device
-        g_color = g_color.contiguous().float()
+        dev = ctx.sigma_rgb.device
+        g_color = _upstream_grad(g_color, ctx.shapes[0], "coarse_raycolor")
+        g_op = _upstream_grad(g_op, ctx.shapes[1], "coarse_point_opacity")
+        g_bg = _upstream_grad(g_bg, ctx.shapes[2], "coarse_is_background")
         N = npnts.xyz.shape[0]
         outs = []
         for need, shape in zip(ctx.needs, ((1, N, 32), (1, N, 3), (1, N, 3), (1, N, 1))):
@@ -331,7 +351,8 @@ class _RenderFn(torch.autograd.Function):
         # (fp32-faithful LeakyReLU masks) | 2 (diagnostic) three-part split in every tensor-core GEMM
         flags = int(getattr(mod.opt, "pnb_bwd_fp32", 0))
         _lib.check(lib.pnb_shade_backward(_lib.C.byref(q.desc), _lib.C.byref(pts), _lib.C.byref(mlp), _lib.C.byref(ctx.o),
-                                          ctx.sigma_rgb.data_ptr(), g_color.data_ptr(), int(ctx.n_valid), int(ctx.n_pairs), ptr(outs[0]),
+                                          ctx.sigma_rgb.data_ptr(), ptr(g_color), ptr(g_op), ptr(g_bg), int(ctx.n_valid),
+                                          int(ctx.n_pairs), ptr(outs[0]),
                                           ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), wp, bp, mod._bwd_ws.data_ptr(),
                                           mod._bwd_ws.numel(), flags, mod._bwd_err.data_ptr(), stream), "pnb_shade_backward")
         grads = []
@@ -639,7 +660,9 @@ class NeuralPointsRayMarching(nn.Module):
             or getattr(opt, "prob", 0) != 0                       # point_aggregators.py:812-813
         if want_aux and inds.shape[0] > 0 and getattr(opt, "prob", 0) != 1:
             # weight / conf_coefficient / blend_weight of the reference dict (:325-329): one kernel on the compacted query
-            wgt, conf_coefficient, blend = _AuxFn.apply(self, q, inds, opacity, npnts.points_conf)
+            # blend_weight is detached (as in the reference), so the kernel's opacity input carries no graph: a loss on conf_coefficient
+            # alone must not reach the shading backward
+            wgt, conf_coefficient, blend = _AuxFn.apply(self, q, inds, opacity.detach(), npnts.points_conf)
             out["weight"] = wgt[None]
             out["blend_weight"] = blend[None, ..., None]
             out["conf_coefficient"] = conf_coefficient[None]
