@@ -49,7 +49,8 @@ typedef enum {
 
 #define PNB_MAX_K 8    /* query_worldcoords.cu:14 (#define KN 8) */
 #define PNB_MAX_SR 128 /* sample slots per ray */
-#define PNB_FEAT 32    /* point_features_dim of every shipped script */
+#define PNB_FEAT 32    /* point_features_dim of most shipped scripts (the default of pnb_points_t.feat_dim) */
+#define PNB_FEAT_DTU 63 /* point_features_dim of the DTU scripts (point_{conf,dir,color}_mode "01": colour, dir, conf + 56 image features) */
 
 /* counters written by pnb_grid_build (device int32[16], copied to host on request) */
 enum {
@@ -123,16 +124,19 @@ typedef struct {
                               * (every shipped script; 0 is read as 2); 1 = alpha_branch on the K-aggregated feature */
 } pnb_shade_opts_t;
 
-/* MLP parameters, fp32, W^T layout [in][out] (transposed once per optimiser step by the host side). */
+/* MLP parameters, fp32, W^T layout [in][out] (transposed once per optimiser step by the host side), zero padded to K_pad rows.
+ * block1.0 takes 7F + 60 inputs [f (F), PE3(f) (6F), PE5(dists) (60)] (point_aggregators.py:278-280): K_pad 288 for F = 32, 512 for
+ * F = 63. */
 typedef struct {
     const float* w[9]; /* block1.0 block1.2 block3.0 block3.2 alpha_branch.0 color_branch.0 .2 .4 .6 */
     const float* b[9];
+    int32_t feat_dim;  /* F the block1.0 weights were built for (32 or 63; 0 is read as 32); must equal the points' */
 } pnb_mlp_t;
 
 /* Neural point attributes (the reference's parameter tensors, read in place). */
 typedef struct {
     const float* xyz;   /* [N,3] */
-    const float* emb;   /* [N,32] points_embeding */
+    const float* emb;   /* [N,feat_dim] points_embeding */
     const float* color; /* [N,3] */
     const float* dir;   /* [N,3] */
     const float* conf;  /* [N]   */
@@ -141,6 +145,7 @@ typedef struct {
                          * scenes (run/editing.py) give each point its own frame: a pair's dists and dir use its point's frame, the
                          * view direction of a sample (PE(view) and every pair's extras) the frame of its slot-0 neighbour
                          * (point_aggregators.py:491-496, :506, :526, :566).  No gradient flows to it. */
+    int32_t feat_dim;   /* point_features_dim F: 32 or 63 (0 is read as 32); any other width is PNB_ERR_UNSUPPORTED */
 } pnb_points_t;
 
 int pnb_version(void);
@@ -196,12 +201,13 @@ int pnb_aux_conf_backward(const pnb_query_t* q, const long long* d_rows, int n_r
 
 /* ---- shading forward on the tensor cores (wgmma, BF16x3 error-compensated split) ---- */
 /* Packs block1 / block3 / colour-branch weights of a pnb_mlp_t (fp32 W^T buffers) into wgmma operand images (hi/lo bf16, one
- * [N x 16] image pair per K step in the shared-memory operand layout).  Call once per weight version.  d_out: >= pnb_mlp_pack_bytes() bytes. */
-size_t pnb_mlp_pack_bytes(void);
+ * [N x 16] image pair per K step in the shared-memory operand layout).  Call once per weight version.  d_out: >= pnb_mlp_pack_bytes(F)
+ * bytes, F = mlp->feat_dim (block1.0: 18 K = 16 steps for F = 32, 32 for F = 63; 0 is read as 32). */
+size_t pnb_mlp_pack_bytes(int feat_dim);
 int pnb_mlp_pack(const pnb_mlp_t* mlp, void* d_out, size_t out_bytes, pnb_stream_t stream);
-/* Frozen point cloud (rendering): the 224 point-only inputs [f, PE3(f)] of block1.0
- * (models/aggregators/point_aggregators.py:547-571) are hoisted out of the per-pair work into a per-point table
- * d_pre[N][256] = b1 + W1[:, :224] . [f_n, PE3(f_n)] (fp32).  Call once per (points_embeding, block1.0) version. */
+/* Frozen point cloud (rendering): the 7F point-only inputs [f, PE3(f)] of block1.0 (224 for F = 32, 441 for F = 63;
+ * models/aggregators/point_aggregators.py:547-571) are hoisted out of the per-pair work into a per-point table
+ * d_pre[N][256] = b1 + W1[:, :7F] . [f_n, PE3(f_n)] (fp32).  Call once per (points_embeding, block1.0) version. */
 size_t pnb_point_pre_bytes(int N);
 int pnb_point_pre(const pnb_points_t* pts, const pnb_mlp_t* mlp, float* d_pre, size_t pre_bytes, pnb_stream_t stream);
 enum {
@@ -210,7 +216,8 @@ enum {
     PNB_TC_FROZEN = 4,          /* pair kernel of a frozen cloud (k_shade_wg<FROZEN>): needs d_point_pre */
     PNB_TC_FEW_CTAS = 2048      /* test of the persistent tile loop: one CTA per 8 SMs instead of one per SM (same results) */
 };
-/* Same contract as pnb_shade_forward; the MLPs run as wgmma tiles.  mlp->w[5] must be zero padded to 288 rows.
+/* Same contract as pnb_shade_forward; the MLPs run as wgmma tiles.  mlp->w[5] must be zero padded to 288 rows; d_packed holds the images
+ * of pnb_mlp_pack for the same F.
  * ws >= pnb_shade_tc_bytes(max_valid_samples).  d_err: device int32[>= 1], 0 on success, 9 if the query produced more valid
  * samples than max_valid_samples (the extra samples are dropped: their sigma_rgb is zeroed, every other result is exact),
  * any other non-zero value = an internal pipeline time-out (a bounded 2-s mbarrier wait expired; results invalid). */
@@ -229,7 +236,7 @@ int pnb_shade_tc_tables(void* ws, size_t ws_bytes, int max_valid_samples, void**
  * (models/mvs_points_volumetric_model.py:98-118): given d(loss)/d(ray_color) [R,3], d(loss)/d(opacity) [R,SR] and
  * d(loss)/d(bg_T) [R] (the full-R layout of pnb_composite_forward; each may be NULL, at least one is given; NULL means that output
  * is not in the loss, and with d_ray_color alone the call is the colour-only backward) accumulates gradients of
- * points_embeding [N,32], points_color [N,3], points_dir [N,3],
+ * points_embeding [N,F], points_color [N,3], points_dir [N,3],
  * points_conf [N] (any may be NULL) and of the 9 MLP layers in the layout of pnb_mlp_t (W^T [K_pad][N] and bias; the
  * caller zero-initialises all accumulators).  d_sigma_rgb_fwd: the forward's per-candidate (sigma, rgb) buffer.
  * n_valid / n_pairs: host copies of counters[PNB_QC_N_VALID] / [PNB_QC_N_PAIRS] (the pair-level buffers hold one row per valid pair).  ws >= pnb_backward_bytes.  The activations are recomputed and every layer
@@ -241,7 +248,7 @@ enum {
     PNB_BWD_FP32_GEMM = 1,      /* every GEMM on the fp32 CUDA-core tiles (parity reference of the tensor-core engine) */
     PNB_BWD_FP32_RECOMPUTE = 4  /* forward recompute on the fp32 tiles (LeakyReLU masks of an fp32 forward), dX / dW on the tensor cores */
 };
-size_t pnb_backward_bytes(int n_valid, int cap_samples);
+size_t pnb_backward_bytes(int n_valid, int cap_samples, int feat_dim /* F of the points; 0 is read as 32 */);
 int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts, const pnb_mlp_t* mlp, const pnb_shade_opts_t* opts,
                        const float* d_sigma_rgb_fwd, const float* d_ray_color /* [R,3] or NULL */,
                        const float* d_opacity /* [R,SR] or NULL */, const float* d_bg_T /* [R] or NULL */, int n_valid, int n_pairs,

@@ -2,7 +2,7 @@
 
 The reference writes, per saved iteration (`/root/reference/models/base_model.py:85-103`):
   `{epoch}_net_ray_marching.pth`  = `net_ray_marching.state_dict()` (after unwrapping `nn.DataParallel`): flat dict
-      neural_points.xyz [N,3] | neural_points.points_embeding [1,N,32] | neural_points.points_conf [1,N,1] |
+      neural_points.xyz [N,3] | neural_points.points_embeding [1,N,F] (F = point_features_dim: 32, or 63 for the DTU scripts) | neural_points.points_conf [1,N,1] |
       neural_points.points_dir [1,N,3] | neural_points.points_color [1,N,3] | (neural_points.eulers, neural_points.Rw2c [3,3] or [N,3,3]) |
       aggregator.{block1.0,block1.2,block3.0,block3.2,alpha_branch.0,color_branch.0,.2,.4,.6}.{weight,bias}
   `{epoch}_states.pth`            = free-form dict of runner state (`epoch_count`, `total_steps`, optimiser states ...)
@@ -89,7 +89,7 @@ def load_into(net, path_or_dict, strict=True):
     np_ = net.neural_points
     np_.set_points(sd["neural_points.xyz"].to(dev), sd["neural_points.points_embeding"].to(dev),
                    points_color=sd["neural_points.points_color"].to(dev), points_dir=sd["neural_points.points_dir"].to(dev),
-                   points_conf=sd["neural_points.points_conf"].to(dev), parameter=True,
+                   points_conf=sd["neural_points.points_conf"].to(dev), parameter=True, as_stored=True,
                    Rw2c=sd["neural_points.Rw2c"].to(dev) if "neural_points.Rw2c" in sd else None)
     agg_sd = {k[len("aggregator."):]: v for k, v in sd.items() if k.startswith("aggregator.")}
     want = set(net.aggregator.state_dict().keys())

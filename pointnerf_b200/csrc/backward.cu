@@ -6,7 +6,7 @@
 //   index_select     /root/reference/models/neural_points/neural_points.py:706-717 (backward = index_add into [1,N,.])
 // Gradients consumed: d loss / d ray_color [R,3], d loss / d opacity [R,SR] and d loss / d bg_T [R] (the outputs ray_march keeps in the
 // autograd graph, returned as coarse_raycolor / coarse_point_opacity / coarse_is_background, neural_points_volumetric_model.py:312-324),
-// each optional.  Gradients produced: points_embeding [N,32], points_color [N,3], points_dir [N,3], points_conf [N] (through
+// each optional.  Gradients produced: points_embeding [N,F] (F = 32 | 63), points_color [N,3], points_dir [N,3], points_conf [N] (through
 // weight*conf_coefficient, straight-through clamp :722-724), and the 18 MLP tensors (in the W^T layout of pnb_mlp_t).
 // xyz receives no gradient (xyz_grad = 0 in every shipped script).
 //
@@ -110,7 +110,8 @@ struct GemmCtx {
     bool fp32_recompute;   // PNB_BWD_FP32_RECOMPUTE: the forward recompute on the fp32 CUDA-core tiles (fp32-faithful LeakyReLU masks)
 };
 constexpr int SPLITK_MAX = 64;
-constexpr size_t PART_FLOATS = (size_t)SPLITK_MAX * 288 * 256;
+// split-K partials of the widest dW GEMM (block1.0: kpad1_of(F) x 256)
+static size_t part_floats(int F) { return (size_t)SPLITK_MAX * kpad1_of(F) * 256; }
 
 __global__ void __launch_bounds__(256) k_lrelu_bwd(float* __restrict__ dY, const float* __restrict__ Y, long ldy, long ldd, int M, int N);
 
@@ -227,7 +228,7 @@ struct BwdParams {
     const uint32_t* pair_off;   // [S+1] first row of every valid sample
     int* row_samp;      // [P] valid-sample index of every row
     // forward recompute buffers
-    float* X1;          // [P x 288]
+    float* X1;          // [P x kpad1_of(F)]  block1.0 inputs
     float* H1;          // [P x 256]
     float* X3;          // [P x 272]  (H2 | extras | 0)
     float* H3;          // [P x 256]
@@ -241,7 +242,7 @@ struct BwdParams {
     float* C1; float* C2; float* C3;   // [S x 128]
     float* O3;          // [S x 4]   raw colour outputs (3 used)
     // gradient buffers
-    float* G1;          // [P x 288]
+    float* G1;          // [P x kpad1_of(F)]  (also scratch of ld 288 for the block3 gradients)
     float* G2;          // [P x 272]
     float* G3;          // [P x 256]
     float* GS1;         // [S x 288]
@@ -260,7 +261,7 @@ __global__ void __launch_bounds__(256) k_bwd_counts(pnb_query_t q, int n_valid, 
 }
 // One warp per valid sample, 4 lanes per pair row: the fp32 forward's row builder, writing the dense block1 input, the block3 extras
 // and the view PE to the recompute buffers.
-template <bool PP>
+template <bool PP, int F>
 __global__ void __launch_bounds__(256) k_bwd_build(BwdParams p) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= p.n_valid) return;
@@ -274,7 +275,7 @@ __global__ void __launch_bounds__(256) k_bwd_build(BwdParams p) {
     if (lane < 8) cx[280 + lane] = 0.f;
     if (!pr.g.valid) return;
     if (part == 0) { p.wc[row] = pr.wc; p.wn[row] = pr.wn; p.pidx[row] = pr.pidx; p.row_samp[row] = vi; }
-    fp32_pair_row<PP>(p.pts, p.o, pr, lane, p.X1 + row * 288, er);
+    fp32_pair_row<PP, F>(p.pts, p.o, pr, lane, p.X1 + row * kpad1_of(F), er);
     if (part == 1)
         for (int e = 7; e < 16; ++e) er[e] = 0.f;
 }
@@ -460,10 +461,11 @@ __global__ void __launch_bounds__(128) k_dw_small(const float* __restrict__ X, l
     }
 }
 
-// Scatter to the points: embedding (through PE), colour, dir, conf.  4 lanes per pair row.
-template <bool PP>
+// Scatter to the points: embedding (through PE), colour, dir, conf.  4 lanes per pair row (8 embedding channels per lane, 16 for F = 63).
+template <bool PP, int F>
 __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* __restrict__ dwc, float* __restrict__ d_emb,
                                                      float* __restrict__ d_color, float* __restrict__ d_dir, float* __restrict__ d_conf) {
+    constexpr int CPL = F == PNB_FEAT ? 8 : 16;
     const long gt = (long)blockIdx.x * blockDim.x + threadIdx.x;
     const long row = gt >> 2;
     const int part = (int)(gt & 3);
@@ -471,20 +473,21 @@ __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* _
     if (row >= P) return;
     const int pi = p.pidx[row];
     if (pi < 0) return;
-    const float* x = p.X1 + row * 288;
-    const float* g = p.G1 + row * 288;
+    const float* x = p.X1 + row * kpad1_of(F);
+    const float* g = p.G1 + row * kpad1_of(F);
     if (d_emb) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            int c = part * 8 + e;
+        for (int e = 0; e < CPL; ++e) {
+            int c = part * CPL + e;
+            if (F != PNB_FEAT && c >= F) continue;
             float acc = g[c];
 #pragma unroll
             for (int j = 0; j < 3; ++j) {
-                float sn = x[32 + (c * 3 + j) * 2], cs = x[32 + (c * 3 + j) * 2 + 1];
-                float gs = g[32 + (c * 3 + j) * 2], gc = g[32 + (c * 3 + j) * 2 + 1];
+                float sn = x[F + (c * 3 + j) * 2], cs = x[F + (c * 3 + j) * 2 + 1];
+                float gs = g[F + (c * 3 + j) * 2], gc = g[F + (c * 3 + j) * 2 + 1];
                 acc = fmaf((float)(1 << j), cs * gs - sn * gc, acc);
             }
-            atomicAdd(&d_emb[(size_t)pi * PNB_FEAT + c], acc);
+            atomicAdd(&d_emb[(size_t)pi * F + c], acc);
         }
     }
     if (part == 0) {
@@ -579,21 +582,21 @@ struct Layout {
     int* row_samp;
     size_t bytes;
 };
-static Layout carve(void* ws, size_t cap, int max_valid, int cap_samples) {
+static Layout carve(void* ws, size_t cap, int max_valid, int cap_samples, int F) {
     Carver c(ws, cap);
     Layout L;
     size_t S = (size_t)(max_valid > 0 ? max_valid : 1), P = S * PNB_MAX_K;
-    L.X1 = c.take<float>(P * 288); L.H1 = c.take<float>(P * 256); L.X3 = c.take<float>(P * 272);
+    L.X1 = c.take<float>(P * kpad1_of(F)); L.H1 = c.take<float>(P * 256); L.X3 = c.take<float>(P * 272);
     L.H3 = c.take<float>(P * 256); L.H4 = c.take<float>(P * 256);
     L.wc = c.take<float>(P); L.wn = c.take<float>(P); L.sp = c.take<float>(P); L.sg = c.take<float>(P); L.dwc = c.take<float>(P);
     L.pidx = c.take<int>(P);
     L.CX = c.take<float>(S * 288); L.C1 = c.take<float>(S * 128); L.C2 = c.take<float>(S * 128); L.C3 = c.take<float>(S * 128);
     L.O3 = c.take<float>(S * 4);
-    L.G1 = c.take<float>(P * 288); L.G2 = c.take<float>(P * 272); L.G3 = c.take<float>(P * 256);
+    L.G1 = c.take<float>(P * kpad1_of(F)); L.G2 = c.take<float>(P * 272); L.G3 = c.take<float>(P * 256);
     L.GS1 = c.take<float>(S * 288); L.GS2 = c.take<float>(S * 128); L.GS3 = c.take<float>(S * 128);
     L.dO3 = c.take<float>(S * 4); L.dsig = c.take<float>(S);
     L.d_sigma_rgb = c.take<float4>((size_t)(cap_samples > 0 ? cap_samples : 1));
-    L.part = c.take<float>(PART_FLOATS);
+    L.part = c.take<float>(part_floats(F));
     L.nv = c.take<uint32_t>(S); L.pair_off = c.take<uint32_t>(S + 1); L.scan_tmp = c.take<uint32_t>(scan_tmp_elems(S)); L.row_samp = c.take<int>(P);
     L.bytes = align_up(c.off);
     return L;
@@ -605,7 +608,10 @@ static Layout carve(void* ws, size_t cap, int max_valid, int cap_samples) {
 using namespace pnb;
 using namespace pnb::bw;
 
-extern "C" size_t pnb_backward_bytes(int n_valid, int cap_samples) { return carve(nullptr, 0, n_valid, cap_samples).bytes; }
+extern "C" size_t pnb_backward_bytes(int n_valid, int cap_samples, int feat_dim) {
+    const int F = feat_of(feat_dim);
+    return F > 0 ? carve(nullptr, 0, n_valid, cap_samples, F).bytes : 0;
+}
 
 // d_mlp_w[i] / d_mlp_b[i]: gradient accumulators in the layout of pnb_mlp_t (W^T [K_pad][N], bias [N]); the caller
 // zero-initialises them.  Point gradients are accumulated (atomicAdd) into d_emb/d_color/d_dir/d_conf (caller zeroes);
@@ -621,7 +627,10 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
                 "pnb_shade_backward: null argument");
     PNB_REQUIRE(d_ray_color || d_opacity || d_bg_T, PNB_ERR_INVALID,
                 "pnb_shade_backward: no upstream gradient (d_ray_color, d_opacity and d_bg_T are all NULL)");
-    Layout L = carve(ws, ws_bytes, n_valid, q->cap_samples);
+    int F = 0;
+    { const int rc = feat_check(pts, mlp, "pnb_shade_backward", &F); if (rc) return rc; }
+    const int KP1 = kpad1_of(F);
+    Layout L = carve(ws, ws_bytes, n_valid, q->cap_samples, F);
     PNB_REQUIRE(L.bytes <= ws_bytes, PNB_ERR_WORKSPACE, "pnb_shade_backward: workspace %zu < required %zu", ws_bytes, L.bytes);
     // composite backward first (also covers n_valid == 0)
     CompBwdParams cp;
@@ -642,13 +651,14 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     p.GS1 = L.GS1; p.GS2 = L.GS2; p.GS3 = L.GS3; p.dO3 = L.dO3; p.dsig = L.dsig; p.d_sigma_rgb = L.d_sigma_rgb;
     p.wa = mlp->w[4]; p.ba = mlp->b[4];
     const int wb = (S * 32 + 255) / 256;   // one warp per sample
-    GemmCtx cx{(flags & 2) != 0, (flags & PNB_BWD_FP32_GEMM) == 0, L.part, PART_FLOATS * sizeof(float), d_err, st, (flags & PNB_BWD_FP32_RECOMPUTE) != 0};
+    GemmCtx cx{(flags & 2) != 0, (flags & PNB_BWD_FP32_GEMM) == 0, L.part, part_floats(F) * sizeof(float), d_err, st, (flags & PNB_BWD_FP32_RECOMPUTE) != 0};
     PNB_REQUIRE(!cx.tc || d_err, PNB_ERR_INVALID, "pnb_shade_backward: the tensor-core path needs d_err");
     // ---------------- forward recompute ----------------
     const bool pp = pts->rw2c != nullptr;                    // per-point frames
-    if (pp) k_bwd_build<true><<<wb, 256, 0, st>>>(p);
-    else k_bwd_build<false><<<wb, 256, 0, st>>>(p);
-    gemm_nn(cx, L.X1, 288, mlp->w[0], 256, L.H1, 256, P, 256, 288, mlp->b[0], 1);
+    void (*build)(BwdParams) = F == PNB_FEAT ? (pp ? k_bwd_build<true, PNB_FEAT> : k_bwd_build<false, PNB_FEAT>)
+                                             : (pp ? k_bwd_build<true, PNB_FEAT_DTU> : k_bwd_build<false, PNB_FEAT_DTU>);
+    build<<<wb, 256, 0, st>>>(p);
+    gemm_nn(cx, L.X1, KP1, mlp->w[0], 256, L.H1, 256, P, 256, KP1, mlp->b[0], 1);
     gemm_nn(cx, L.H1, 256, mlp->w[1], 256, L.X3, 272, P, 256, 256, mlp->b[1], 1);   // H2 into X3[:, :256]
     gemm_nn(cx, L.X3, 272, mlp->w[2], 256, L.H3, 256, P, 256, 272, mlp->b[2], 1);
     gemm_nn(cx, L.H3, 256, mlp->w[3], 256, L.H4, 256, P, 256, 256, mlp->b[3], 1);
@@ -689,12 +699,15 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     colsum(L.G2, 272, P, 256, d_mlp_b[1], st);
     gemm_nt(cx, L.G2, 272, mlp->w[1], 256, L.G3, 256, P, 256, 256, L.H1, 256, 256);   // dH1 in G3
     // block1.0
-    gemm_tn_acc(cx, L.X1, 288, L.G3, 256, d_mlp_w[0], 256, P, 288, 256);
+    gemm_tn_acc(cx, L.X1, KP1, L.G3, 256, d_mlp_w[0], 256, P, KP1, 256);
     colsum(L.G3, 256, P, 256, d_mlp_b[0], st);
-    gemm_nt(cx, L.G3, 256, mlp->w[0], 256, L.G1, 288, P, 224, 256);                   // dX1: only the 224 feature columns are consumed (k_bwd_scatter; no xyz gradient)
+    // dX1: only the 7F feature columns are consumed (k_bwd_scatter; no xyz gradient), rounded up to 16: 224 | 448
+    gemm_nt(cx, L.G3, 256, mlp->w[0], 256, L.G1, KP1, P, (7 * F + 15) / 16 * 16, 256);
     // scatter to the points
-    if (pp) k_bwd_scatter<true><<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
-    else k_bwd_scatter<false><<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
+    void (*scatter)(BwdParams, const float*, float*, float*, float*, float*) =
+        F == PNB_FEAT ? (pp ? k_bwd_scatter<true, PNB_FEAT> : k_bwd_scatter<false, PNB_FEAT>)
+                      : (pp ? k_bwd_scatter<true, PNB_FEAT_DTU> : k_bwd_scatter<false, PNB_FEAT_DTU>);
+    scatter<<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }

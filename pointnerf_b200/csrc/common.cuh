@@ -31,6 +31,24 @@ void set_error(const char* fmt, ...);
 
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
+// ---- point_features_dim F: 32 (most shipped scripts) or 63 (the DTU scripts), each a compile-time instantiation of the kernels
+// F (0 read as 32) or -1 when the width has no instantiation
+static inline int feat_of(int32_t f) { return f == 0 ? PNB_FEAT : (f == PNB_FEAT || f == PNB_FEAT_DTU) ? (int)f : -1; }
+// block1.0 inputs [f (F), PE3(f) (6F), PE5(dists) (60)] = 7F + 60, padded to whole K = 32 blocks: 288 | 512
+__host__ __device__ constexpr int kpad1_of(int F) { return F == PNB_FEAT ? 288 : 512; }
+// The points' F (0 read as 32), which must have an instantiation and, with an MLP, equal the MLP's.  Sets the error text on failure.
+static inline int feat_check(const pnb_points_t* pts, const pnb_mlp_t* mlp, const char* fn, int* F) {
+    const int fp = feat_of(pts->feat_dim);
+    PNB_REQUIRE(fp > 0, PNB_ERR_UNSUPPORTED, "%s: point_features_dim %d unsupported (32 or 63)", fn, (int)pts->feat_dim);
+    if (mlp) {
+        const int fm = feat_of(mlp->feat_dim);
+        PNB_REQUIRE(fm == fp, PNB_ERR_INVALID, "%s: the MLP was built for point_features_dim %d, the points have %d", fn,
+                    (int)(mlp->feat_dim ? mlp->feat_dim : PNB_FEAT), fp);
+    }
+    *F = fp;
+    return PNB_OK;
+}
+
 // Bump allocator over a caller-provided workspace.
 struct Carver {
     char* base;

@@ -255,7 +255,8 @@ static GridLayout carve_grid(void* buf, size_t cap, int N, const int32_t dim[3])
 
 using namespace pnb;
 
-extern "C" int pnb_version(void) { return 102; }   // 101: pnb_points_t.rw2c; 102: pnb_shade_backward takes d_opacity, d_bg_T
+extern "C" int pnb_version(void) { return 103; }   // 101: pnb_points_t.rw2c; 102: pnb_shade_backward takes d_opacity, d_bg_T;
+                                                   // 103: pnb_points_t / pnb_mlp_t.feat_dim (F = 32 | 63), F-sized *_bytes()
 extern "C" const char* pnb_last_error(void) { return pnb::g_err; }
 extern "C" size_t pnb_struct_size(int which) {
     switch (which) {

@@ -179,9 +179,10 @@ __device__ __forceinline__ float ray_dist_step(const pnb_query_t& q, const pnb_s
 //   fp32_pair      the sample, the pair geometry and the weights; lanes 0-11 write the sample's view encoding PE4 (ori=True
 //                  layout, index d*4 + j: networks.py:183): sin to vpe[0..11], cos to vpe[12..23].  have: the warp has a sample s;
 //                  nk: slots k < nk are read from cand_pidx
-//   fp32_pair_row  for a non-empty slot, the row's four lanes write the 288 block1.0 inputs to xr (features (32), PE3 of the
-//                  features (192, index (c*3 + j)*2 + {sin, cos}), PE5 of the dists (60), 4 zeros); part 1 writes the 7 block3
-//                  extras to ex
+//   fp32_pair_row  for a non-empty slot, the row's four lanes write the kpad1_of(F) block1.0 inputs to xr (features (F), PE3 of the
+//                  features (6F, index F + (c*3 + j)*2 + {sin, cos}), PE5 of the dists (60, from column 7F), zeros up to 288 | 512);
+//                  part 1 writes the 7 block3 extras to ex.  F = 63: emb rows are not 16-byte aligned (scalar loads), 16 channels
+//                  per lane
 struct Fp32Pair {
     PairGeom g;
     int pidx;
@@ -217,25 +218,38 @@ __device__ __forceinline__ Fp32Pair fp32_pair(const pnb_query_t& q, const pnb_po
     r.wc = r.g.valid ? r.wn * r.g.cc : 0.f;
     return r;
 }
-template <bool PP>
+template <bool PP, int F = PNB_FEAT>
 __device__ __forceinline__ void fp32_pair_row(const pnb_points_t& pts, const pnb_shade_opts_t& o, const Fp32Pair& r, int lane, float* xr,
                                               float* ex) {
+    static_assert(F == PNB_FEAT || F == PNB_FEAT_DTU, "point_features_dim 32 or 63");
+    constexpr int CPL = F == PNB_FEAT ? 8 : 16;   // channels per lane
+    constexpr int DC = 7 * F;                     // first column of the distance PE
     const int part = lane & 3;
     const PairGeom& g = r.g;
-    // features: this lane's 8 channels + their PE (3 freqs)
-    const float4* ep = (const float4*)&pts.emb[(size_t)g.pi * PNB_FEAT + part * 8];
-    const float4 f0 = __ldg(ep), f1 = __ldg(ep + 1);
-    const float f[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
+    // features: this lane's channels + their PE (3 freqs)
+    float f[CPL];
+    if (F == PNB_FEAT) {
+        const float4* ep = (const float4*)&pts.emb[(size_t)g.pi * F + part * 8];
+        const float4 f0 = __ldg(ep), f1 = __ldg(ep + 1);
+        f[0] = f0.x; f[1] = f0.y; f[2] = f0.z; f[3] = f0.w; f[4] = f1.x; f[5] = f1.y; f[6] = f1.z; f[7] = f1.w;
+    } else {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-        const int c = part * 8 + e;
+        for (int e = 0; e < CPL; ++e) {
+            const int c = part * CPL + e;
+            f[e] = c < F ? __ldg(&pts.emb[(size_t)g.pi * F + c]) : 0.f;
+        }
+    }
+#pragma unroll
+    for (int e = 0; e < CPL; ++e) {
+        const int c = part * CPL + e;
+        if (F != PNB_FEAT && c >= F) continue;
         xr[c] = f[e];
 #pragma unroll
         for (int j = 0; j < 3; ++j) {
             float sn, cn;
             sincosf(f[e] * (float)(1 << j), &sn, &cn);
-            xr[32 + (c * 3 + j) * 2] = sn;
-            xr[32 + (c * 3 + j) * 2 + 1] = cn;
+            xr[F + (c * 3 + j) * 2] = sn;
+            xr[F + (c * 3 + j) * 2 + 1] = cn;
         }
     }
     // distance PE (5 freqs): 30 (d, j) pairs split over the 4 lanes
@@ -244,10 +258,14 @@ __device__ __forceinline__ void fp32_pair_row(const pnb_points_t& pts, const pnb
         const int dd = i / 5, jj = i - dd * 5;
         float sn, cn;
         sincosf(dist[dd] * (float)(1 << jj), &sn, &cn);
-        xr[224 + i * 2] = sn;
-        xr[224 + i * 2 + 1] = cn;
+        xr[DC + i * 2] = sn;
+        xr[DC + i * 2 + 1] = cn;
     }
-    if (part == 0) { xr[284] = 0.f; xr[285] = 0.f; xr[286] = 0.f; xr[287] = 0.f; }
+    if (F == PNB_FEAT) {
+        if (part == 0) { xr[284] = 0.f; xr[285] = 0.f; xr[286] = 0.f; xr[287] = 0.f; }
+    } else {
+        for (int c = DC + 60 + part; c < kpad1_of(F); c += 4) xr[c] = 0.f;
+    }
     if (part == 1) point_extras<PP>(pts, o, g.pi, r.ov, ex);
 }
 

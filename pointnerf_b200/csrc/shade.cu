@@ -14,6 +14,8 @@
 // Tile = 8 valid samples x 8 neighbour slots = 64 (sample,k) pair rows; one warp builds one sample's rows.
 // Activations never leave shared memory; weights (W^T, zero padded to multiples of 16 rows) stream from L2
 // through a cp.async double buffer.
+// F = 63 (point_features_dim of the DTU scripts): the 512-wide block1.0 input rows (stride XS1) overlay X and H, which are contiguous;
+// layer 1 writes H only after its last read of the rows (gemm64x256 synchronises before its epilogue).
 #include "pair_inputs.cuh"
 
 namespace pnb {
@@ -22,6 +24,7 @@ constexpr int TS = 8;             // samples per tile
 constexpr int TR = TS * PNB_MAX_K;  // 64 pair rows
 constexpr int XS = 292;           // X row stride (floats): 284 inputs padded to 288, +4 against bank conflicts
 constexpr int HS = 284;           // H row stride: holds 280 colour-branch inputs (256 + 24) and 272 block3 inputs
+constexpr int XS1 = 516;          // F = 63: block1.0 input row stride (512 inputs + 4), over X and H
 constexpr int KC = 16;            // weight rows per pipeline stage
 constexpr int NTHREADS = 256;
 constexpr float LEAKY = 0.01f;
@@ -152,11 +155,15 @@ __device__ __forceinline__ void dense8(const float* __restrict__ in, int sin_, f
     __syncthreads();
 }
 
-// PP: per-point frames (pts.rw2c != NULL), a compile-time parameter
-template <bool PP>
+static_assert(offsetof(ShadeSmem, H) == sizeof(float) * TR * XS && TR * XS1 <= TR * (XS + HS), "F = 63 rows overlay X and H");
+
+// PP: per-point frames (pts.rw2c != NULL); F: point_features_dim (32 | 63); both compile-time parameters
+template <bool PP, int F>
 __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     ShadeSmem& sm = *reinterpret_cast<ShadeSmem*>(smem_raw);
+    constexpr int KP1 = kpad1_of(F), XS_1 = F == PNB_FEAT ? XS : XS1;    // block1.0 inputs: width, row stride
+    float* const X1 = reinterpret_cast<float*>(smem_raw);                  // == sm.X (F = 63: over sm.H as well)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_valid = p.q.counters[PNB_QC_N_VALID];
     const int n_tiles = (n_valid + TS - 1) / TS;
@@ -170,15 +177,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
             const int row = warp * PNB_MAX_K + k;
             const bool have = vi < n_valid;
             const uint32_t s = have ? q.valid_list[vi] : 0xffffffffu;
-            float* xr = &sm.X[row * XS];
+            float* xr = &X1[row * XS_1];
             if (lane == 0) sm.samp[warp] = s;
             const Fp32Pair pr = fp32_pair<PP>(q, p.pts, p.o, have, s, q.K, lane, &sm.view[warp][3]);
             if (lane < 3) sm.view[warp][lane] = lane == 0 ? pr.ov.x : lane == 1 ? pr.ov.y : pr.ov.z;
             if (part == 0) sm.wc[row] = pr.wc;
             if (pr.g.valid) {
-                fp32_pair_row<PP>(p.pts, p.o, pr, lane, xr, sm.E[row]);
+                fp32_pair_row<PP, F>(p.pts, p.o, pr, lane, xr, sm.E[row]);
             } else {
-                for (int c = part; c < 288; c += 4) xr[c] = 0.f;
+                for (int c = part; c < KP1; c += 4) xr[c] = 0.f;
                 if (part == 1)
                     for (int e = 0; e < 7; ++e) sm.E[row][e] = 0.f;
             }
@@ -186,7 +193,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
         }
         __syncthreads();
         // ------------------------------------------------------------------ phase B: per-pair MLPs
-        gemm64x256(sm.X, XS, sm.H, HS, p.mlp.w[0], p.mlp.b[0], 288, sm.W, true);   // block1.0  284 -> 256
+        gemm64x256(X1, XS_1, sm.H, HS, p.mlp.w[0], p.mlp.b[0], KP1, sm.W, true);   // block1.0  7F + 60 -> 256
         gemm64x256(sm.H, HS, sm.X, XS, p.mlp.w[1], p.mlp.b[1], 256, sm.W, true);   // block1.2  256 -> 256
         for (int i = tid; i < TR * 16; i += NTHREADS) {                             // cat extras, zero pad to 272
             int row = i >> 4, c = i & 15;
@@ -403,21 +410,26 @@ extern "C" int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, 
     PNB_REQUIRE(q->K >= 1 && q->K <= PNB_MAX_K, PNB_ERR_UNSUPPORTED, "pnb_shade_forward: K=%d unsupported", q->K);
     for (int i = 0; i < 9; ++i)
         PNB_REQUIRE(mlp->w[i] && mlp->b[i], PNB_ERR_INVALID, "pnb_shade_forward: MLP tensor %d is null", i);
+    int F = 0;
+    { const int rc = feat_check(pts, mlp, "pnb_shade_forward", &F); if (rc) return rc; }
     static int smem_set[64] = {0}, n_sm_of[64] = {0};      // per device of this process
     int dev = 0;
     PNB_CHECK_CUDA(cudaGetDevice(&dev));
     PNB_REQUIRE(dev >= 0 && dev < 64, PNB_ERR_UNSUPPORTED, "pnb_shade_forward: device ordinal %d", dev);
     if (!smem_set[dev]) {
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false, PNB_FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true, PNB_FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false, PNB_FEAT_DTU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true, PNB_FEAT_DTU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
         PNB_CHECK_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
         smem_set[dev] = 1;
     }
     const int n_sm = n_sm_of[dev];
     ShadeParams p;
     p.q = *q; p.pts = *pts; p.mlp = *mlp; p.o = *opts; p.sigma_rgb = (float4*)d_sigma_rgb;
-    if (pts->rw2c) k_shade_fwd<true><<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
-    else k_shade_fwd<false><<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
+    void (*kern)(ShadeParams) = F == PNB_FEAT ? (pts->rw2c ? k_shade_fwd<true, PNB_FEAT> : k_shade_fwd<false, PNB_FEAT>)
+                                              : (pts->rw2c ? k_shade_fwd<true, PNB_FEAT_DTU> : k_shade_fwd<false, PNB_FEAT_DTU>);
+    kern<<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }
@@ -440,6 +452,8 @@ extern "C" int pnb_aux_outputs(const pnb_query_t* q, const pnb_points_t* pts, co
     cudaStream_t stream = (cudaStream_t)stream_;
     PNB_REQUIRE(q && pts && d_opacity && d_weight && d_conf_coefficient && d_blend_weight, PNB_ERR_INVALID, "pnb_aux_outputs: null argument");
     PNB_REQUIRE(q->K >= 1 && q->K <= PNB_MAX_K, PNB_ERR_UNSUPPORTED, "pnb_aux_outputs: K=%d unsupported", q->K);
+    int F = 0;
+    { const int rc = feat_check(pts, nullptr, "pnb_aux_outputs", &F); if (rc) return rc; }
     if (n_rows <= 0) return PNB_OK;
     PNB_REQUIRE(d_rows, PNB_ERR_INVALID, "pnb_aux_outputs: null row list");
     AuxParams p;

@@ -27,9 +27,22 @@ constexpr int LAYOUT = LAYOUT_NONE;
 constexpr int TM = 128;                 // pair rows per tile
 constexpr int ABLK = 128 * 64;          // bytes of one A block ([128 x 32] bf16)
 constexpr int NKB_MAX = 9;
-__host__ __device__ constexpr int nkb_of(int l) { return (l == 0 || l == 2) ? 9 : 8; }
-__host__ __device__ constexpr int img_base(int l) { return l == 0 ? 0 : l == 1 ? 9 : l == 2 ? 17 : 26; }  // in K blocks
-constexpr int NBLK_TOTAL = 34;
+// K blocks of block1.0 (9 | 16 for F = 32 | 63), of layer l, and the first K block of layer l in the packed images
+__host__ __device__ constexpr int nkb0_of(int F) { return kpad1_of(F) / 32; }
+__host__ __device__ constexpr int nkb_of(int l, int F = PNB_FEAT) { return l == 0 ? nkb0_of(F) : l == 2 ? 9 : 8; }
+__host__ __device__ constexpr int img_base(int l, int F = PNB_FEAT) { return l == 0 ? 0 : l == 1 ? nkb0_of(F) : l == 2 ? nkb0_of(F) + 8 : nkb0_of(F) + 17; }
+__host__ __device__ constexpr int nblk_total(int F) { return nkb0_of(F) + 25; }
+// F = 63: the 512 block1.0 inputs are built and multiplied in two halves of 256 operand columns (the whole row, 128 rows x hi / lo,
+// would take 256 KB).  Operand column order (the packer maps the W^T rows to it, w1_row_f63):
+//   half 0:  PE5(dists) (60) + 4 zeros | PE3 of channels 0..31 (6 per channel: 2j + {sin, cos})
+//   half 1:  raw features 0..62 + 1 zero | PE3 of channels 32..62 + 6 zeros
+// so that the frozen kernel's distance-only layer 1 is K steps 0..3, and the second half needs no pair geometry.
+__host__ __device__ inline int w1_row_f63(int k) {     // W^T row (reference input order) of operand column k; -1: zero
+    if (k < 64) return k < 60 ? 7 * PNB_FEAT_DTU + k : -1;
+    if (k < 256) return PNB_FEAT_DTU + (k - 64);
+    if (k < 320) return k - 256 < PNB_FEAT_DTU ? k - 256 : -1;
+    return 32 + (k - 320) / 6 < PNB_FEAT_DTU ? PNB_FEAT_DTU + 6 * 32 + (k - 320) : -1;
+}
 constexpr int STEP = 2 * 256 * 32;      // one weight stage: hi + lo image ([256 x 16] bf16 each) of one K = 16 step
 constexpr float LEAKY = 0.01f;
 constexpr int XE = 128 * 32;            // bytes of one [128 x 16] bf16 extras operand (SBO = 256)
@@ -102,29 +115,43 @@ __device__ __forceinline__ float seg_sum8(float v, int lane, int st, int cnt) {
 // FROZEN (part 1 only, one builder thread per row): the feature columns come from the per-point table, so the row is part 1
 // without the feature PE and with the distance PE at operand columns 0..63 (K blocks 0, 1); it also records the row's point.
 // PP: per-point frames (pair_inputs.cuh, point_frame).
-template <int PART, bool FROZEN, bool PP, class SmemT>
+// F = 63 (not FROZEN; column order at tc::w1_row_f63), half HALF of the row:
+//   half 0: part 0 = PE of features 0..23; part 1 = PE of features 24..31, PE of the distances, extras, weight*conf, the row's point
+//   half 1: part 0 = raw features, PE of features 32..43; part 1 = PE of features 44..62 (the point is read back from sm.prow)
+// emb rows of 63 floats are not 16-byte aligned: scalar loads.
+template <int PART, bool FROZEN, bool PP, int F = PNB_FEAT, int HALF = 0, class SmemT>
 __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& p, int row, int n_valid, int pvi, int pk, int pst, int pcnt) {
     using namespace tc;
     static_assert(PART == 0 || PART == 1, "two parts per row");
     static_assert(!FROZEN || PART == 1, "the frozen row is a part-1 row");
+    constexpr bool W = F != PNB_FEAT;                                   // the 512-wide row of F = 63
+    static_assert(!W || (F == PNB_FEAT_DTU && !FROZEN && (HALF == 0 || HALF == 1)), "F = 63: two halves, not frozen");
+    static_assert(W || HALF == 0, "F = 32: one row");
     constexpr bool P0 = PART == 0, P1 = PART == 1;
-    constexpr int G_LO = P0 ? 0 : 5, G_HI = (P1 && !FROZEN) ? 8 : 5;   // feature groups (4 features each) whose PE this part builds
-    constexpr int DCOL = FROZEN ? 0 : 224;                              // first operand column of the distance PE
-    constexpr int C_LO = P1 && !FROZEN ? 19 : 0, C_HI = P0 ? 19 : FROZEN ? 8 : 36;   // 16-byte chunks (column / 8) of this part
+    constexpr bool GEO = P1 && HALF == 0;                               // forms the pair geometry: dist PE, extras, weight*conf
+    constexpr bool RAW = P0 && (!W || HALF == 1);                       // writes the raw features
+    constexpr int G_LO = !W ? (P0 ? 0 : 5) : HALF == 0 ? (P0 ? 0 : 6) : (P0 ? 8 : 11);   // feature groups (4 features each) whose
+    constexpr int G_HI = !W ? ((P1 && !FROZEN) ? 8 : 5) : HALF == 0 ? (P0 ? 6 : 8) : (P0 ? 11 : 16);   // PE this part builds
+    constexpr int GCOL0 = !W ? 32 : 64 - 192 * HALF;                    // operand column of group gi: GCOL0 + 24 gi
+    constexpr int NRAW = W ? 8 : 4;                                     // 16-byte chunks of raw features
+    constexpr int DCOL = (FROZEN || W) ? 0 : 224;                       // first operand column of the distance PE
+    constexpr int C_LO = P1 && !FROZEN ? 19 : 0, C_HI = P0 ? 19 : FROZEN ? 8 : 36;   // 16-byte chunks (column / 8) of this part (F = 32)
     const pnb_query_t& q = p.q;
     int pidx = -1, p0 = 0;
     CandSample cs = {};
-    if (pvi >= 0 && pvi < n_valid) {
+    if (W && HALF == 1) {
+        pidx = sm.prow[row];
+    } else if (pvi >= 0 && pvi < n_valid) {
         const uint32_t s = q.valid_list[pvi];
-        if (P1) { cs = cand_sample(q, s); p0 = view_point<PP>(q, s); }
+        if (GEO) { cs = cand_sample(q, s); p0 = view_point<PP>(q, s); }
         if (pk < q.K) pidx = q.cand_pidx[(size_t)s * q.K + pk];
     }
-    if (FROZEN) sm.prow[row] = pidx;
+    if (FROZEN || (W && GEO)) sm.prow[row] = pidx;
     const bool valid = pidx >= 0;
     const int pi = valid ? pidx : 0;
     PairGeom g;
     float3 ov;
-    if (P1) {
+    if (GEO) {
         ov = view_in_points<PP>(p.pts, p.o, p0, cs.dir);
         g = pair_geom<PP>(p.pts, p.o, pidx, cs.pos);
         const float wsum = seg_sum8(g.w, row & 31, pst, pcnt);   // every lane takes part in the shuffles
@@ -132,27 +159,40 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
     }
     float ex[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (valid) {
-        const float4* ep = (const float4*)&p.pts.emb[(size_t)pi * PNB_FEAT];
+        const float4* ep = (const float4*)&p.pts.emb[(size_t)pi * F];
+        const float* es = &p.pts.emb[(size_t)pi * F];
 #pragma unroll
         for (int gi = G_LO; gi < G_HI; ++gi) {  // 4 features per step
-            float4 fv = __ldg(ep + gi);
-            float f[4] = {fv.x, fv.y, fv.z, fv.w};
+            float f[4];
+            if (!W) {
+                float4 fv = __ldg(ep + gi);
+                f[0] = fv.x; f[1] = fv.y; f[2] = fv.z; f[3] = fv.w;
+            } else {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) f[e] = 4 * gi + e < F ? __ldg(es + 4 * gi + e) : 0.f;
+            }
             float pe[24];
 #pragma unroll
             for (int e = 0; e < 4; ++e) pe_doubling<3>(f[e], pe + e * 6);
-            const int col = 32 + 24 * gi;
+            const int col = GCOL0 + 24 * gi;
 #pragma unroll
             for (int c = 0; c < 3; ++c) store_chunk8_a1(sm, row, (col + 8 * c) >> 5, (col + 8 * c) & 31, pe + 8 * c);
         }
-        if (P0) {
+        if (RAW) {
 #pragma unroll
-            for (int gi = 0; gi < 4; ++gi) {    // raw features, 8 per chunk (re-read: L1 hit)
-                float4 a = __ldg(ep + 2 * gi), b = __ldg(ep + 2 * gi + 1);
-                float f8[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-                store_chunk8_a1(sm, row, 0, 8 * gi, f8);
+            for (int gi = 0; gi < NRAW; ++gi) {    // raw features, 8 per chunk (re-read: L1 hit)
+                float f8[8];
+                if (!W) {
+                    float4 a = __ldg(ep + 2 * gi), b = __ldg(ep + 2 * gi + 1);
+                    f8[0] = a.x; f8[1] = a.y; f8[2] = a.z; f8[3] = a.w; f8[4] = b.x; f8[5] = b.y; f8[6] = b.z; f8[7] = b.w;
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) f8[e] = 8 * gi + e < F ? __ldg(es + 8 * gi + e) : 0.f;
+                }
+                store_chunk8_a1(sm, row, (8 * gi) >> 5, (8 * gi) & 31, f8);
             }
         }
-        if (P1) {
+        if (GEO) {
             float dp[64];
 #pragma unroll
             for (int e = 0; e < 6; ++e) pe_doubling<5>(g.dist[e], dp + 10 * e);
@@ -163,9 +203,20 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
         }
     } else {
         float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        for (int c = C_LO; c < C_HI; ++c) store_chunk8_a1(sm, row, c >> 2, (c & 3) * 8, z8);
+        if (!W) {
+            for (int c = C_LO; c < C_HI; ++c) store_chunk8_a1(sm, row, c >> 2, (c & 3) * 8, z8);
+        } else {
+#pragma unroll
+            for (int c = 3 * G_LO; c < 3 * G_HI; ++c) store_chunk8_a1(sm, row, (GCOL0 + 8 * c) >> 5, (GCOL0 + 8 * c) & 31, z8);
+            if (RAW)
+#pragma unroll
+                for (int c = 0; c < NRAW; ++c) store_chunk8_a1(sm, row, (8 * c) >> 5, (8 * c) & 31, z8);
+            if (GEO)
+#pragma unroll
+                for (int c = 0; c < 8; ++c) store_chunk8_a1(sm, row, (DCOL + 8 * c) >> 5, (DCOL + 8 * c) & 31, z8);
+        }
     }
-    if (P1) {   // block3 extras operand [128 x 16]: chunk 0 = extras, chunk 1 = 0
+    if (GEO) {   // block3 extras operand [128 x 16]: chunk 0 = extras, chunk 1 = 0
         uint32_t h[4], l[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) split_bf16x2(ex[2 * i], ex[2 * i + 1], h[i], l[i]);
@@ -186,6 +237,21 @@ __global__ void __launch_bounds__(256) k_pack_weights(const float* __restrict__ 
     const int n = rem >> 4, k = rem & 15;
     const int kg = ks * 16 + k;
     const float v = kg < Kpad ? wt[(size_t)kg * N + n] : 0.f;
+    __nv_bfloat16 h, l;
+    split_bf16(v, h, l);
+    const uint32_t off = k16_offset_bytes(n, k);
+    const size_t img = (size_t)N * 32;
+    *(__nv_bfloat16*)(out + (size_t)(2 * ks) * img + off) = h;
+    *(__nv_bfloat16*)(out + (size_t)(2 * ks + 1) * img + off) = l;
+}
+// block1.0 of F = 63: the same images, operand column kg taken from W^T row tc::w1_row_f63(kg)
+__global__ void __launch_bounds__(256) k_pack_block1_f63(const float* __restrict__ wt, int nks, int N, unsigned char* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;   // (ks, n, k)
+    if (i >= nks * N * 16) return;
+    const int ks = i / (N * 16), rem = i - ks * N * 16;
+    const int n = rem >> 4, k = rem & 15;
+    const int src = tc::w1_row_f63(ks * 16 + k);
+    const float v = src >= 0 ? wt[(size_t)src * N + n] : 0.f;
     __nv_bfloat16 h, l;
     split_bf16(v, h, l);
     const uint32_t off = k16_offset_bytes(n, k);
@@ -406,38 +472,44 @@ __device__ __forceinline__ QuadRow quad_row(uint32_t head, int tot, int lane) {
     return r;
 }
 
-// pre[n][c] = b1[c] + sum_{k<224} W1^T[k][c] * x_n[k],  x_n = [f (32), PE3(f) (192, column 32 + 6*feature + 2*j + {sin, cos})]:
-// exactly the first 7 K blocks of the operand build_pair_part writes.  fp32 FMAs in ascending k.  Block = 32 points x 256 columns.
+// pre[n][c] = b1[c] + sum_{k<7F} W1^T[k][c] * x_n[k],  x_n = [f (F), PE3(f) (6F, column F + 6*feature + 2*j + {sin, cos})]: the
+// point-only inputs of block1.0 (F = 32: exactly the first 7 K blocks of the operand build_pair_part writes).  fp32 FMAs in ascending k.
+// Block = NP points x 256 columns (F = 63: 16 points, the 441 inputs padded to 444 with zeros).
+template <int F>
 __global__ void __launch_bounds__(256) k_point_pre(const float* __restrict__ emb, int N, const float* __restrict__ w1t, const float* __restrict__ b1,
                                                    float* __restrict__ pre) {
-    __shared__ __align__(16) float x[32][224 + 4];
-    const int n0 = blockIdx.x * 32;
-    for (int i = threadIdx.x; i < 32 * PNB_FEAT; i += 256) {
-        const int pl = i >> 5, f = i & 31, n = n0 + pl;
-        const float v = n < N ? __ldg(&emb[(size_t)n * PNB_FEAT + f]) : 0.f;
+    constexpr int NP = F == PNB_FEAT ? 32 : 16;           // points per block
+    constexpr int KX = (7 * F + 3) / 4 * 4;               // inputs, whole float4: 224 | 444
+    __shared__ __align__(16) float x[NP][KX + 4];
+    const int n0 = blockIdx.x * NP;
+    for (int i = threadIdx.x; i < NP * F; i += 256) {
+        const int pl = F == PNB_FEAT ? i >> 5 : i / F, f = F == PNB_FEAT ? i & 31 : i - pl * F, n = n0 + pl;
+        const float v = n < N ? __ldg(&emb[(size_t)n * F + f]) : 0.f;
         float pe[6];
         pe_doubling<3>(v, pe);
         x[pl][f] = v;
 #pragma unroll
-        for (int e = 0; e < 6; ++e) x[pl][32 + 6 * f + e] = pe[e];
+        for (int e = 0; e < 6; ++e) x[pl][F + 6 * f + e] = pe[e];
     }
+    if (KX > 7 * F)
+        for (int i = threadIdx.x; i < NP * (KX - 7 * F); i += 256) x[i / (KX - 7 * F)][7 * F + i % (KX - 7 * F)] = 0.f;
     __syncthreads();
     const int c = threadIdx.x;
-    float acc[32];
+    float acc[NP];
     const float bc = __ldg(&b1[c]);
 #pragma unroll
-    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-    for (int k = 0; k < 224; k += 4) {
+    for (int i = 0; i < NP; ++i) acc[i] = 0.f;
+    for (int k = 0; k < KX; k += 4) {
         const float w0 = __ldg(&w1t[(size_t)k * 256 + c]), w1 = __ldg(&w1t[(size_t)(k + 1) * 256 + c]);
         const float w2 = __ldg(&w1t[(size_t)(k + 2) * 256 + c]), w3 = __ldg(&w1t[(size_t)(k + 3) * 256 + c]);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
+        for (int i = 0; i < NP; ++i) {
             const float4 xv = *reinterpret_cast<const float4*>(&x[i][k]);
             acc[i] = fmaf(xv.w, w3, fmaf(xv.z, w2, fmaf(xv.y, w1, fmaf(xv.x, w0, acc[i]))));
         }
     }
 #pragma unroll
-    for (int i = 0; i < 32; ++i)
+    for (int i = 0; i < NP; ++i)
         if (n0 + i < N) pre[(size_t)(n0 + i) * 256 + c] = acc[i] + bc;
 }
 
@@ -458,7 +530,8 @@ namespace hw {
 constexpr int NTHR = 256;
 constexpr int NSTAGE = 4;
 constexpr int YLD = 260;                  // fp32 row stride of the last-epilogue buffer: lane = row float4 reads are conflict-free
-constexpr int KS_FROZEN0 = 14;            // first K step of the frozen layer 1 (operand columns 224..287 of block1.0)
+// first K step of the frozen layer 1: the distance PE (F = 32: operand columns 224..287 of block1.0; F = 63: 0..63, tc::w1_row_f63)
+__host__ __device__ constexpr int ks_frozen0(int F) { return F == PNB_FEAT ? 14 : 0; }
 struct Smem {
     unsigned char a_hi[tc::NKB_MAX * tc::ABLK];   // layer operand; a_hi + a_lo also hold the fp32 [128 x YLD] rows of the last epilogue
     unsigned char a_lo[tc::NKB_MAX * tc::ABLK];
@@ -472,23 +545,27 @@ struct Smem {
     uint64_t bar_full[NSTAGE], bar_empty[NSTAGE];
 };
 static_assert(tc::TM * YLD * 4 <= 2 * tc::NKB_MAX * tc::ABLK, "last-epilogue rows exceed the operand region");
-// K = 16 steps of a tile: layer 1 (18 | FROZEN 4), layer 2 (16), layer 3 (16 + the extras step), layer 4 (16)
-__host__ __device__ constexpr int steps_of(int l, bool frozen) { return l == 0 ? (frozen ? 4 : 18) : l == 2 ? 17 : 16; }
+// K = 16 steps of a tile: layer 1 (18 | F = 63: 32 | FROZEN 4), layer 2 (16), layer 3 (16 + the extras step), layer 4 (16)
+__host__ __device__ constexpr int steps_of(int l, bool frozen, int F = PNB_FEAT) { return l == 0 ? (frozen ? 4 : kpad1_of(F) / 16) : l == 2 ? 17 : 16; }
 // weight image (index in K = 16 steps of the packed pair images) of step j of a tile
+template <int F = PNB_FEAT>
 __device__ __forceinline__ uint32_t step_image(uint32_t j, bool frozen) {
-    const uint32_t s0 = (uint32_t)steps_of(0, frozen);
-    if (j < s0) return (frozen ? (uint32_t)KS_FROZEN0 : 0u) + j;
+    const uint32_t s0 = (uint32_t)steps_of(0, frozen, F);
+    if (j < s0) return (frozen ? (uint32_t)ks_frozen0(F) : 0u) + j;
     j -= s0;
-    if (j < 16u) return 2u * tc::img_base(1) + j;
+    if (j < 16u) return 2u * tc::img_base(1, F) + j;
     j -= 16u;
-    if (j < 17u) return 2u * tc::img_base(2) + j;
-    return 2u * tc::img_base(3) + (j - 17u);
+    if (j < 17u) return 2u * tc::img_base(2, F) + j;
+    return 2u * tc::img_base(3, F) + (j - 17u);
 }
 }  // namespace hw
 
 // O1: agg_intrp_order == 1 as a compile-time flag (the alpha dot product over the K-aggregated feature); PP: per-point frames
-// (pts.rw2c != NULL), compile-time as well, so that the uniform-frame builds keep their registers
-template <bool FROZEN, bool O1, bool PP>
+// (pts.rw2c != NULL), compile-time as well, so that the uniform-frame builds keep their registers; F: point_features_dim (32 | 63).
+// F = 63, not FROZEN: layer 1 runs over 512 operand columns in two halves of 16 K steps; after the first half every wgmma that read it
+// retires (both warpgroups), the builders write the second half over it and the accumulator carries on.  FROZEN does not read the
+// features: only its layer-1 weight images differ.
+template <bool FROZEN, bool O1, bool PP, int F>
 __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -500,7 +577,8 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
     const int n_quads = p.pack_cnt[0];
     const int n_tiles = (n_quads + 3) >> 2;
     const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-    constexpr uint32_t ST = (uint32_t)(hw::steps_of(0, FROZEN) + 16 + 17 + 16);
+    constexpr bool SPLIT = F != PNB_FEAT && !FROZEN;              // layer 1 in two halves
+    constexpr uint32_t ST = (uint32_t)(hw::steps_of(0, FROZEN, F) + 16 + 17 + 16);
 
     if (tid == 0) {
         for (int s = 0; s < hw::NSTAGE; ++s) { mbar_init(&sm.bar_full[s], 1); mbar_init(&sm.bar_empty[s], hw::NTHR / 32); }
@@ -508,7 +586,7 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
         if (blockIdx.x == 0 && q.counters[PNB_QC_N_VALID] > p.hbar_cap) atomicExch(p.err, 9);
     }
     __syncthreads();
-    auto img_of = [](uint32_t m) { return hw::step_image(m % ST, FROZEN); };
+    auto img_of = [](uint32_t m) { return hw::step_image<F>(m % ST, FROZEN); };
     Ring<hw::NSTAGE, STEP, decltype(img_of)> ring{sm.b, sm.bar_full, sm.bar_empty, p.wimg, (uint32_t)my_tiles * ST, img_of, p.err};
     if (tid == 0) ring.prologue();
 
@@ -541,17 +619,32 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
                 if (lane == 0 && part == 0) { sm.qhead[qw] = head; sm.qfirst[qw] = first; sm.qtotal[qw] = (uint32_t)total; }
                 const int pvi = qr.live ? (int)p.vorder[first + qr.j] : -1;
                 if (FROZEN) build_pair_part<1, true, PP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else if (part == 0) build_pair_part<0, false, PP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else build_pair_part<1, false, PP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else if (part == 0) build_pair_part<0, false, PP, F>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else build_pair_part<1, false, PP, F>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
             }
             fence_proxy_async();
             named_bar_sync(1, hw::NTHR);
         }
         // ---------------- the four layers
         for (int l = 0; l < 4; ++l) {
-            const int nst = hw::steps_of(l, FROZEN);
+            const int nst = hw::steps_of(l, FROZEN, F);
             wg::fence();
             for (int kk = 0; kk < nst; ++kk, ++m) {
+                if constexpr (SPLIT) {
+                    if (l == 0 && kk == 16) {
+                        // second half of the layer-1 operand: the first half's wgmma have retired in both warpgroups before it is
+                        // overwritten (its last weight stage is released after the next step, as usual)
+                        wg::wait<0>();
+                        pin<128>(acc);
+                        named_bar_sync(1, hw::NTHR);
+                        const int row = (warp & 3) * 32 + lane;
+                        if (warp < 4) build_pair_part<0, false, PP, F, 1>(sm, p, row, n_valid, -1, 0, 0, 1);
+                        else build_pair_part<1, false, PP, F, 1>(sm, p, row, n_valid, -1, 0, 0, 1);
+                        fence_proxy_async();
+                        named_bar_sync(1, hw::NTHR);
+                        wg::fence();
+                    }
+                }
                 ok = ring.acquire(m, ok);
                 const uint32_t bs = b0 + (m % hw::NSTAGE) * (uint32_t)STEP;
                 const uint64_t bh = desc_k16(bs), bl = desc_k16(bs + STEP / 2);
@@ -559,7 +652,8 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
                 if (l == 2 && kk == 16) {
                     ah = desc_k16(xe_hi0); al = desc_k16(xe_lo0);
                 } else {
-                    const uint32_t off = (uint32_t)(kk >> 1) * ABLK + (uint32_t)(kk & 1) * 256u;
+                    const int ka = SPLIT && l == 0 ? (kk & 15) : kk;      // K step within the operand in shared memory
+                    const uint32_t off = (uint32_t)(ka >> 1) * ABLK + (uint32_t)(ka & 1) * 256u;
                     ah = desc_none(a_hi0 + off); al = desc_none(a_lo0 + off);
                 }
                 mma_n256(acc, ah, bh, kk ? 1u : 0u);
@@ -844,26 +938,33 @@ __global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
 
 using namespace pnb;
 
-static size_t pack_pairs_bytes() { return (size_t)tc::NBLK_TOTAL * 2 * tc::STEP; }
+static size_t pack_pairs_bytes(int F) { return (size_t)tc::nblk_total(F) * 2 * tc::STEP; }
 static size_t pack_color_bytes() { return (size_t)ctc::NBLK * 2 * hcw::STEP; }
-extern "C" size_t pnb_mlp_pack_bytes(void) { return pack_pairs_bytes() + pack_color_bytes(); }
+extern "C" size_t pnb_mlp_pack_bytes(int feat_dim) {
+    const int F = feat_of(feat_dim);
+    return F > 0 ? pack_pairs_bytes(F) + pack_color_bytes() : 0;
+}
 
 // Packs block1/block3 and colour_branch.{0,2,4} weights (pnb_mlp_t W^T buffers, fp32) into wgmma operand images, one hi + lo
 // pair per K = 16 step.  Call once per weight version.
 extern "C" int pnb_mlp_pack(const pnb_mlp_t* mlp, void* d_out, size_t out_bytes, pnb_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     PNB_REQUIRE(mlp && d_out, PNB_ERR_INVALID, "pnb_mlp_pack: null argument");
-    PNB_REQUIRE(out_bytes >= pnb_mlp_pack_bytes(), PNB_ERR_WORKSPACE, "pnb_mlp_pack: buffer too small");
-    const int kpad[4] = {288, 256, 272, 256};
+    const int F = feat_of(mlp->feat_dim);
+    PNB_REQUIRE(F > 0, PNB_ERR_UNSUPPORTED, "pnb_mlp_pack: point_features_dim %d unsupported (32 or 63)", (int)mlp->feat_dim);
+    PNB_REQUIRE(out_bytes >= pnb_mlp_pack_bytes(F), PNB_ERR_WORKSPACE, "pnb_mlp_pack: buffer too small");
+    const int kpad[4] = {kpad1_of(F), 256, 272, 256};
     for (int l = 0; l < 4; ++l) {
-        const int nks = 2 * tc::nkb_of(l), n = nks * 256 * 16;
-        k_pack_weights<<<(n + 255) / 256, 256, 0, stream>>>(mlp->w[l], kpad[l], nks, 256, (unsigned char*)d_out + (size_t)tc::img_base(l) * 2 * tc::STEP);
+        const int nks = 2 * tc::nkb_of(l, F), n = nks * 256 * 16;
+        unsigned char* dst = (unsigned char*)d_out + (size_t)tc::img_base(l, F) * 2 * tc::STEP;
+        if (l == 0 && F != PNB_FEAT) k_pack_block1_f63<<<(n + 255) / 256, 256, 0, stream>>>(mlp->w[0], nks, 256, dst);
+        else k_pack_weights<<<(n + 255) / 256, 256, 0, stream>>>(mlp->w[l], kpad[l], nks, 256, dst);
     }
     const int ckpad[3] = {288, 128, 128};   // colour_branch.{0,2,4}: W^T [K_pad][128]
     for (int l = 0; l < 3; ++l) {
         const int nks = 2 * ctc::nkb_of(l), n = nks * 128 * 16;
         k_pack_weights<<<(n + 255) / 256, 256, 0, stream>>>(mlp->w[5 + l], ckpad[l], nks, 128,
-                                                            (unsigned char*)d_out + pack_pairs_bytes() + (size_t)ctc::img_base(l) * 2 * hcw::STEP);
+                                                            (unsigned char*)d_out + pack_pairs_bytes(F) + (size_t)ctc::img_base(l) * 2 * hcw::STEP);
     }
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
@@ -875,7 +976,10 @@ extern "C" int pnb_point_pre(const pnb_points_t* pts, const pnb_mlp_t* mlp, floa
     cudaStream_t stream = (cudaStream_t)stream_;
     PNB_REQUIRE(pts && mlp && d_pre, PNB_ERR_INVALID, "pnb_point_pre: null argument");
     PNB_REQUIRE(pre_bytes >= pnb_point_pre_bytes(pts->N), PNB_ERR_WORKSPACE, "pnb_point_pre: buffer too small");
-    if (pts->N > 0) k_point_pre<<<(pts->N + 31) / 32, 256, 0, stream>>>(pts->emb, pts->N, mlp->w[0], mlp->b[0], d_pre);
+    int F = 0;
+    { const int rc = feat_check(pts, mlp, "pnb_point_pre", &F); if (rc) return rc; }
+    if (pts->N > 0 && F == PNB_FEAT) k_point_pre<PNB_FEAT><<<(pts->N + 31) / 32, 256, 0, stream>>>(pts->emb, pts->N, mlp->w[0], mlp->b[0], d_pre);
+    else if (pts->N > 0) k_point_pre<PNB_FEAT_DTU><<<(pts->N + 15) / 16, 256, 0, stream>>>(pts->emb, pts->N, mlp->w[0], mlp->b[0], d_pre);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }
@@ -924,6 +1028,8 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
     PNB_REQUIRE(ws_bytes >= pnb_shade_tc_bytes(max_valid_samples), PNB_ERR_WORKSPACE, "pnb_shade_forward_tc: workspace too small");
     const bool frozen = (flags & PNB_TC_FROZEN) != 0;
     PNB_REQUIRE(!frozen || d_point_pre, PNB_ERR_INVALID, "pnb_shade_forward_tc: PNB_TC_FROZEN needs the table of pnb_point_pre");
+    int F = 0;
+    { const int rc = feat_check(pts, mlp, "pnb_shade_forward_tc", &F); if (rc) return rc; }
     static int configured[64] = {0}, n_sm_of[64] = {0};      // per device of this process (one process per GPU is the norm)
     int dev = 0;
     PNB_CHECK_CUDA(cudaGetDevice(&dev));
@@ -934,10 +1040,15 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
     static_assert(sizeof(hw::Smem) + 128 <= kSmemMax, "pair kernel shared-memory carve-out exceeds the per-block limit");
     static_assert(sizeof(hcw::Smem) + 128 <= kSmemMax, "colour kernel shared-memory carve-out exceeds the per-block limit");
     if (!configured[dev]) {
-        const void* pair_kernels[8] = {(const void*)k_shade_wg<false, false, false>, (const void*)k_shade_wg<false, true, false>,
-                                       (const void*)k_shade_wg<true, false, false>, (const void*)k_shade_wg<true, true, false>,
-                                       (const void*)k_shade_wg<false, false, true>, (const void*)k_shade_wg<false, true, true>,
-                                       (const void*)k_shade_wg<true, false, true>, (const void*)k_shade_wg<true, true, true>};
+        const void* pair_kernels[16] = {
+            (const void*)k_shade_wg<false, false, false, PNB_FEAT>, (const void*)k_shade_wg<false, true, false, PNB_FEAT>,
+            (const void*)k_shade_wg<true, false, false, PNB_FEAT>, (const void*)k_shade_wg<true, true, false, PNB_FEAT>,
+            (const void*)k_shade_wg<false, false, true, PNB_FEAT>, (const void*)k_shade_wg<false, true, true, PNB_FEAT>,
+            (const void*)k_shade_wg<true, false, true, PNB_FEAT>, (const void*)k_shade_wg<true, true, true, PNB_FEAT>,
+            (const void*)k_shade_wg<false, false, false, PNB_FEAT_DTU>, (const void*)k_shade_wg<false, true, false, PNB_FEAT_DTU>,
+            (const void*)k_shade_wg<true, false, false, PNB_FEAT_DTU>, (const void*)k_shade_wg<true, true, false, PNB_FEAT_DTU>,
+            (const void*)k_shade_wg<false, false, true, PNB_FEAT_DTU>, (const void*)k_shade_wg<false, true, true, PNB_FEAT_DTU>,
+            (const void*)k_shade_wg<true, false, true, PNB_FEAT_DTU>, (const void*)k_shade_wg<true, true, true, PNB_FEAT_DTU>};
         for (const void* k : pair_kernels) PNB_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
@@ -963,15 +1074,19 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
         const bool o1 = opts->agg_intrp_order == 1;              // compile-time flags of the kernel
         const bool pp = pts->rw2c != nullptr;
         void (*kern)(ShadeTcParams) =
-            frozen ? (o1 ? (pp ? k_shade_wg<true, true, true> : k_shade_wg<true, true, false>)
-                         : (pp ? k_shade_wg<true, false, true> : k_shade_wg<true, false, false>))
-                   : (o1 ? (pp ? k_shade_wg<false, true, true> : k_shade_wg<false, true, false>)
-                         : (pp ? k_shade_wg<false, false, true> : k_shade_wg<false, false, false>));
+            F == PNB_FEAT ? (frozen ? (o1 ? (pp ? k_shade_wg<true, true, true, PNB_FEAT> : k_shade_wg<true, true, false, PNB_FEAT>)
+                                          : (pp ? k_shade_wg<true, false, true, PNB_FEAT> : k_shade_wg<true, false, false, PNB_FEAT>))
+                                    : (o1 ? (pp ? k_shade_wg<false, true, true, PNB_FEAT> : k_shade_wg<false, true, false, PNB_FEAT>)
+                                          : (pp ? k_shade_wg<false, false, true, PNB_FEAT> : k_shade_wg<false, false, false, PNB_FEAT>)))
+                          : (frozen ? (o1 ? (pp ? k_shade_wg<true, true, true, PNB_FEAT_DTU> : k_shade_wg<true, true, false, PNB_FEAT_DTU>)
+                                          : (pp ? k_shade_wg<true, false, true, PNB_FEAT_DTU> : k_shade_wg<true, false, false, PNB_FEAT_DTU>))
+                                    : (o1 ? (pp ? k_shade_wg<false, true, true, PNB_FEAT_DTU> : k_shade_wg<false, true, false, PNB_FEAT_DTU>)
+                                          : (pp ? k_shade_wg<false, false, true, PNB_FEAT_DTU> : k_shade_wg<false, false, false, PNB_FEAT_DTU>)));
         kern<<<n_cta, hw::NTHR, smem_pair, stream>>>(p);
     }
     if (flags & PNB_TC_COLOR) {
         ColorTcParams ct;
-        ct.q = *q; ct.o = *opts; ct.wimg = (const unsigned char*)d_packed + pack_pairs_bytes();
+        ct.q = *q; ct.o = *opts; ct.wimg = (const unsigned char*)d_packed + pack_pairs_bytes(F);
         for (int i = 0; i < 3; ++i) ct.bias[i] = mlp->b[5 + i];
         ct.w3t = mlp->w[8]; ct.b3 = mlp->b[8];
         ct.hbar = w.hbar; ct.sigma = w.sigma; ct.hbar_cap = max_valid_samples; ct.sigma_rgb = (float4*)d_sigma_rgb; ct.err = d_err;

@@ -7,8 +7,9 @@ from . import scene
 from .ray_marching import NeuralPoints, NeuralPointsRayMarching, PointAggregator
 
 
-def make_opt(cfg, is_train=False, **over):
-    """The option surface the hot path reads (SURVEY.md 8b), with the shipped values (section 8 head)."""
+def make_opt(cfg, is_train=False, feat_dim=32, **over):
+    """The option surface the hot path reads (SURVEY.md 8b), with the shipped values (section 8 head).  feat_dim 63: the DTU
+    scripts' point_features_dim 63 with point_{conf,dir,color}_mode "01"."""
     o = SimpleNamespace(
         # querier (point_query.py:33-42,76-93)
         inverse=0, radius_limit_scale=cfg.radius_limit_scale, vsize=[cfg.vsize] * 3, vscale=[cfg.vscale] * 3,
@@ -28,16 +29,20 @@ def make_opt(cfg, is_train=False, **over):
         # ray marcher
         raydist_mode_unit=1, which_render_func="radiance", which_blend_func="alpha", which_tonemap_func="off",
     )
+    if feat_dim != 32:
+        o.point_features_dim = feat_dim
+        o.point_conf_mode = o.point_dir_mode = o.point_color_mode = "01"
     for k, v in over.items():
         setattr(o, k, v)
     return o
 
 
-def build_model(cfg, device, seed=0, alpha_bias=0.0, is_train=False, **over):
+def build_model(cfg, device, seed=0, alpha_bias=0.0, is_train=False, feat_dim=32, **over):
     """Returns (net, points_cpu_dict, opt).  MLP init seed `seed`; alpha_bias raises alpha_branch.0.bias
-    to make the scene opaque (a more discriminating parity case, SURVEY section 7)."""
-    opt = make_opt(cfg, is_train=is_train, **over)
-    pts = scene.make_points(cfg)
+    to make the scene opaque (a more discriminating parity case, SURVEY section 7).  feat_dim 63: the DTU configuration (56 image
+    features, colour, dir and conf prepended by set_points)."""
+    opt = make_opt(cfg, is_train=is_train, feat_dim=feat_dim, **over)
+    pts = scene.make_points(cfg, emb_dim=32 if feat_dim == 32 else feat_dim - 7)
     agg = PointAggregator(opt, seed=seed)
     with torch.no_grad():
         agg.alpha_branch[0].bias += alpha_bias

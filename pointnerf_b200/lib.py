@@ -43,12 +43,12 @@ class ShadeOpts(C.Structure):
 
 
 class Mlp(C.Structure):
-    _fields_ = [("w", C.c_void_p * 9), ("b", C.c_void_p * 9)]
+    _fields_ = [("w", C.c_void_p * 9), ("b", C.c_void_p * 9), ("feat_dim", C.c_int32)]
 
 
 class Points(C.Structure):
     _fields_ = [("xyz", C.c_void_p), ("emb", C.c_void_p), ("color", C.c_void_p), ("dir", C.c_void_p),
-                ("conf", C.c_void_p), ("N", C.c_int32), ("rw2c", C.c_void_p)]
+                ("conf", C.c_void_p), ("N", C.c_int32), ("rw2c", C.c_void_p), ("feat_dim", C.c_int32)]
 
 
 GC = dict(n_occ=0, max_pts=1, overflow_o=2, overflow_p=3, n_inrange=4, slot0_cell=5, first_pt=6)
@@ -117,7 +117,7 @@ def load():
     lib.pnb_aux_conf_backward.restype = C.c_int
     lib.pnb_aux_conf_backward.argtypes = [C.POINTER(Query), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.pnb_mlp_pack_bytes.restype = C.c_size_t
-    lib.pnb_mlp_pack_bytes.argtypes = []
+    lib.pnb_mlp_pack_bytes.argtypes = [C.c_int]
     lib.pnb_mlp_pack.restype = C.c_int
     lib.pnb_mlp_pack.argtypes = [C.POINTER(Mlp), C.c_void_p, C.c_size_t, C.c_void_p]
     lib.pnb_point_pre_bytes.restype = C.c_size_t
@@ -133,7 +133,7 @@ def load():
     lib.pnb_shade_tc_tables.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                         C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     lib.pnb_backward_bytes.restype = C.c_size_t
-    lib.pnb_backward_bytes.argtypes = [C.c_int, C.c_int]
+    lib.pnb_backward_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.pnb_shade_backward.restype = C.c_int
     lib.pnb_shade_backward.argtypes = [C.POINTER(Query), C.POINTER(Points), C.POINTER(Mlp), C.POINTER(ShadeOpts), C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

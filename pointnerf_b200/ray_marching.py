@@ -26,14 +26,36 @@ MLP_KEYS = ("block1.0", "block1.2", "block3.0", "block3.2", "alpha_branch.0",
             "color_branch.0", "color_branch.2", "color_branch.4", "color_branch.6")
 MLP_SHAPES = ((256, 284), (256, 256), (256, 263), (256, 256), (1, 256), (128, 280), (128, 128), (128, 128), (3, 128))
 MLP_KPAD = (288, 256, 272, 256, 256, 288, 128, 128, 128)  # rows of the W^T buffers handed to the kernels
+# point_features_dim values with a kernel instantiation: 32 (most shipped scripts) and 63 (the DTU scripts)
+FEAT_DIMS = (32, 63)
+POINT_MODES = ("1", "01")   # point_{conf,dir,color}_mode: "0" also prepends the tensor to the embedding (NeuralPoints.set_points)
+
+
+def mlp_shapes(F=32):
+    """(out, in) of the 9 MLP tensors for point_features_dim F: block1.0 takes 7F + 60 inputs (point_aggregators.py:278-280)."""
+    return ((256, 7 * F + 60),) + MLP_SHAPES[1:]
+
+
+def mlp_kpad(F=32):
+    """Rows of the W^T buffers for point_features_dim F (block1.0: 288 | 512)."""
+    return ((288 if F == 32 else 512),) + MLP_KPAD[1:]
+
+
+def feat_dim_of_block1(n_in):
+    """point_features_dim of a block1.0 with n_in inputs (7F + 60); NotImplementedError for a width without kernels."""
+    F, r = divmod(int(n_in) - 60, 7)
+    if r or F not in FEAT_DIMS:
+        raise NotImplementedError("pnb200: block1.0 with %d inputs (point_features_dim %s) is outside the implemented hot path (%s)"
+                                  % (n_in, F if not r else "?", " or ".join(str(7 * f + 60) for f in FEAT_DIMS)))
+    return F
 
 _REQUIRED = dict(
     agg_dist_pers=20, agg_distance_kernel="linear", apply_pnt_mask=1, num_feat_freqs=3,
     dist_xyz_freq=5, dist_xyz_deno=0, num_viewdir_freqs=4, view_ori=0, shading_feature_mlp_layer1=2,
     shading_feature_mlp_layer2=0, shading_feature_mlp_layer3=2, shading_alpha_mlp_layer=1,
     shading_color_mlp_layer=4, shading_feature_num=256, act_type="LeakyReLU", act_super=1,
-    point_features_dim=32, agg_feat_xyz_mode="None", agg_alpha_xyz_mode="None", agg_color_xyz_mode="None",
-    which_agg_model="viewmlp", agg_weight_norm=1, point_conf_mode="1", point_dir_mode="1", point_color_mode="1",
+    agg_feat_xyz_mode="None", agg_alpha_xyz_mode="None", agg_color_xyz_mode="None",
+    which_agg_model="viewmlp", agg_weight_norm=1,
 )
 _DEFAULTS = dict(view_ori=0, act_super=1, agg_weight_norm=1, apply_pnt_mask=1, which_agg_model="viewmlp",
                  dist_xyz_deno=0, agg_feat_xyz_mode="None", agg_alpha_xyz_mode="None", agg_color_xyz_mode="None",
@@ -50,6 +72,14 @@ def check_opt(opt):
             ok = str(have) == str(want)
         if not ok:
             raise NotImplementedError("pnb200: option %s=%r is outside the implemented hot path (needs %r)" % (k, have, want))
+    F = getattr(opt, "point_features_dim", 32)
+    if float(F) not in [float(f) for f in FEAT_DIMS]:
+        raise NotImplementedError("pnb200: option point_features_dim=%r is outside the implemented hot path (needs 32 or 63)" % (F,))
+    for k in ("point_conf_mode", "point_dir_mode", "point_color_mode"):
+        have = str(getattr(opt, k, "1"))
+        if have not in POINT_MODES:
+            # without "1" the tensor is not kept beside the embedding and the shading inputs lack it
+            raise NotImplementedError("pnb200: option %s=%r is outside the implemented hot path (needs '1' or '01')" % (k, have))
     order = int(getattr(opt, "agg_intrp_order", 2))
     if order not in (1, 2):
         # agg_intrp_order 0 (features interpolated before the MLP) does not run in the reference either: viewmlp raises a shape error with
@@ -81,8 +111,9 @@ class PointAggregator(nn.Module):
         if opt is not None:
             check_opt(opt)
         self.opt = opt
+        F = int(getattr(opt, "point_features_dim", 32)) if opt is not None else 32
         act = lambda: nn.LeakyReLU(inplace=True)
-        self.block1 = nn.Sequential(nn.Linear(284, 256), act(), nn.Linear(256, 256), act())
+        self.block1 = nn.Sequential(nn.Linear(7 * F + 60, 256), act(), nn.Linear(256, 256), act())
         self.block3 = nn.Sequential(nn.Linear(263, 256), act(), nn.Linear(256, 256), act())
         self.alpha_branch = nn.Sequential(nn.Linear(256, 1))
         self.color_branch = nn.Sequential(nn.Linear(280, 128), act(), nn.Linear(128, 128), act(),
@@ -117,8 +148,9 @@ class MlpPack:
         bs = [sd[k + ".bias"] for k in MLP_KEYS]
         key = tuple((t.data_ptr(), t._version) for t in ws + bs)
         if key != self.key:
+            F = feat_dim_of_block1(ws[0].shape[1])
             self.wt, self.bias = [], []
-            for w, b, shp, kp in zip(ws, bs, MLP_SHAPES, MLP_KPAD):
+            for w, b, shp, kp in zip(ws, bs, mlp_shapes(F), mlp_kpad(F)):
                 assert tuple(w.shape) == shp, "MLP tensor shape %s != %s" % (tuple(w.shape), shp)
                 wt = torch.zeros((kp, shp[0]), dtype=torch.float32, device=w.device)
                 wt[:shp[1]].copy_(w.detach().t())
@@ -128,12 +160,13 @@ class MlpPack:
             for i in range(9):
                 d.w[i] = self.wt[i].data_ptr()
                 d.b[i] = self.bias[i].data_ptr()
+            d.feat_dim = F
             self.desc = d
             self.key = key
             self.key_l1 = (key[0], key[9])
             lib = _lib.load()
-            nb = lib.pnb_mlp_pack_bytes()
-            if self.packed is None or self.packed.device != ws[0].device:
+            nb = lib.pnb_mlp_pack_bytes(F)
+            if self.packed is None or self.packed.device != ws[0].device or self.packed.numel() != nb:
                 self.packed = torch.empty(nb, dtype=torch.uint8, device=ws[0].device)
             _lib.check(lib.pnb_mlp_pack(_lib.C.byref(d), self.packed.data_ptr(), nb,
                                         torch.cuda.current_stream(ws[0].device).cuda_stream), "pnb_mlp_pack")
@@ -159,9 +192,14 @@ def points_desc_of(npnts):
     for t in tens:
         if not (t.is_cuda and t.is_contiguous() and t.dtype == torch.float32):
             raise _lib.PnbError("pnb200: point tensors must be contiguous fp32 CUDA tensors")
-    if npnts.points_embeding.shape[-1] != 32:
-        raise NotImplementedError("pnb200: point_features_dim must be 32")
+    F = int(npnts.points_embeding.shape[-1])
+    if F not in FEAT_DIMS:
+        raise NotImplementedError("pnb200: point_features_dim must be 32 or 63, the embedding has %d channels" % F)
+    want = getattr(getattr(npnts, "opt", None), "point_features_dim", None)
+    if want is not None and int(want) != F:
+        raise _lib.PnbError("pnb200: points_embeding has %d channels, opt.point_features_dim=%d" % (F, int(want)))
     p.xyz, p.emb, p.color, p.dir, p.conf = (t.data_ptr() for t in tens)
+    p.feat_dim = F
     p.N = npnts.xyz.shape[0]
     if per_point_rw2c(npnts):
         if tuple(R.shape) != (p.N, 3, 3) or R.dtype != torch.float32 or not R.is_contiguous() or R.device != npnts.xyz.device:
@@ -197,15 +235,30 @@ class NeuralPoints(nn.Module):
         self.querier = lighting_fast_querier(device, opt)
 
     def set_points(self, points_xyz, points_embeding, points_color=None, points_dir=None, points_conf=None,
-                   parameter=True, Rw2c=None, **_):
-        """neural_points.py:400-467.  Rw2c: None (identity), one [3,3] rotation for the whole cloud, or one per point [N,3,3]."""
+                   parameter=True, Rw2c=None, as_stored=False, **_):
+        """neural_points.py:400-467.  Rw2c: None (identity), one [3,3] rotation for the whole cloud, or one per point [N,3,3].
+        The embedding is cut to opt.point_features_dim; a point_{conf,dir,color}_mode containing "0" prepends that tensor to it (conf,
+        then dir, then colour: [color, dir, conf, emb]), one containing "1" keeps it as its own tensor (the DTU scripts: "01").
+        as_stored: the tensors as a checkpoint holds them (the embedding already complete), installed without either step."""
         mk = (lambda t, g: nn.Parameter(t.contiguous(), requires_grad=g)) if parameter else (lambda t, g: t.contiguous())
         o = self.opt
+        F = int(getattr(o, "point_features_dim", points_embeding.shape[-1]))
+        if as_stored:
+            F = points_embeding.shape[-1]
+        if points_embeding.shape[-1] > F:
+            points_embeding = points_embeding[..., :F]
+        kept = {}
+        for name, t, mode in (("points_conf", points_conf, "point_conf_mode"), ("points_dir", points_dir, "point_dir_mode"),
+                              ("points_color", points_color, "point_color_mode")):
+            m = "1" if as_stored else str(getattr(o, mode, "1"))
+            if t is not None and "0" in m:
+                points_embeding = torch.cat([t, points_embeding], dim=-1)
+            kept[name] = t if "1" in m else None
         self.xyz = mk(points_xyz, getattr(o, "xyz_grad", 0) > 0)
         self.points_embeding = mk(points_embeding, getattr(o, "feat_grad", 1) > 0)
-        self.points_color = mk(points_color, getattr(o, "color_grad", 1) > 0)
-        self.points_dir = mk(points_dir, getattr(o, "dir_grad", 1) > 0)
-        self.points_conf = mk(points_conf, getattr(o, "conf_grad", 1) > 0)
+        self.points_color = None if kept["points_color"] is None else mk(kept["points_color"], getattr(o, "color_grad", 1) > 0)
+        self.points_dir = None if kept["points_dir"] is None else mk(kept["points_dir"], getattr(o, "dir_grad", 1) > 0)
+        self.points_conf = None if kept["points_conf"] is None else mk(kept["points_conf"], getattr(o, "conf_grad", 1) > 0)
         if "Rw2c" in self._parameters:
             del self._parameters["Rw2c"]
         # a supplied Rw2c is part of the state dict, as in the reference (neural_points.py:463-467); the default stays a plain eye(3)
@@ -331,12 +384,13 @@ class _RenderFn(torch.autograd.Function):
         g_op = _upstream_grad(g_op, ctx.shapes[1], "coarse_point_opacity")
         g_bg = _upstream_grad(g_bg, ctx.shapes[2], "coarse_is_background")
         N = npnts.xyz.shape[0]
+        F = int(npnts.points_embeding.shape[-1])
         outs = []
-        for need, shape in zip(ctx.needs, ((1, N, 32), (1, N, 3), (1, N, 3), (1, N, 1))):
+        for need, shape in zip(ctx.needs, ((1, N, F), (1, N, 3), (1, N, 3), (1, N, 1))):
             outs.append(torch.zeros(shape, dtype=torch.float32, device=dev) if need else None)
         dwt = [torch.zeros_like(w) for w in mod._mlp.wt]
         dbs = [torch.zeros_like(b) for b in mod._mlp.bias]
-        nb = lib.pnb_backward_bytes(max(ctx.n_valid, 1), q.desc.cap_samples)
+        nb = lib.pnb_backward_bytes(max(ctx.n_valid, 1), q.desc.cap_samples, F)
         if getattr(mod, "_bwd_ws", None) is None or mod._bwd_ws.numel() < nb:
             mod._bwd_ws = torch.empty(nb, dtype=torch.uint8, device=dev)
         wp = (_lib.C.c_void_p * 9)(*[t.data_ptr() for t in dwt])
@@ -356,8 +410,8 @@ class _RenderFn(torch.autograd.Function):
                                           ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), wp, bp, mod._bwd_ws.data_ptr(),
                                           mod._bwd_ws.numel(), flags, mod._bwd_err.data_ptr(), stream), "pnb_shade_backward")
         grads = []
-        for i, shp in enumerate(MLP_SHAPES):                 # W^T [K_pad, N] -> nn.Linear weight [N, K]
-            grads.append(dwt[i][:shp[1]].t().contiguous().view(ctx.mlp_shapes[2 * i]))
+        for i in range(len(MLP_KEYS)):                       # W^T [K_pad, N] -> nn.Linear weight [N, K]
+            grads.append(dwt[i][:ctx.mlp_shapes[2 * i][1]].t().contiguous().view(ctx.mlp_shapes[2 * i]))
             grads.append(dbs[i].view(ctx.mlp_shapes[2 * i + 1]))
         return (None, None, outs[0], outs[1], outs[2], outs[3], *grads)
 
@@ -709,5 +763,5 @@ class NeuralPointsRayMarching(nn.Module):
             out.update({"ray_max_shading_opacity": torch.zeros([0, 0, 1, 1], device=dev), "ray_max_sample_loc_w": torch.zeros([0, 0, 3], device=dev),
                         "ray_max_far_dist": torch.zeros([0, 0, 1], device=dev), "shading_avg_color": torch.zeros([0, 0, 3], device=dev),
                         "shading_avg_dir": torch.zeros([0, 0, 3], device=dev), "shading_avg_conf": torch.zeros([0, 0, 1], device=dev),
-                        "shading_avg_embedding": torch.zeros([0, 0, 32], device=dev)})
+                        "shading_avg_embedding": torch.zeros([0, 0, int(npnts.points_embeding.shape[-1])], device=dev)})
         return out

@@ -52,8 +52,10 @@ CONFIGS = {
 }
 
 
-def make_points(cfg: SceneConfig, device="cpu"):
-    """xyz[N,3], embedding[1,N,32], color[1,N,3], dir[1,N,3], conf[1,N,1], Rw2c[3,3] (fp32)."""
+def make_points(cfg: SceneConfig, device="cpu", emb_dim=32):
+    """xyz[N,3], embedding[1,N,emb_dim], color[1,N,3], dir[1,N,3], conf[1,N,1], Rw2c[3,3] (fp32).  emb_dim 32 (the default) gives
+    the seeded values of every existing fixture; the DTU configuration (point_features_dim 63, point_*_mode "01") takes 56 image
+    features and prepends colour, dir and conf itself (NeuralPoints.set_points)."""
     g = torch.Generator().manual_seed(cfg.seed)
     N = cfg.N
     if cfg.shape == "shell":
@@ -80,7 +82,7 @@ def make_points(cfg: SceneConfig, device="cpu"):
             xyz[m, oth[0]] = u[m, 0] * 2 * half[oth[0]]
             xyz[m, oth[1]] = u[m, 1] * 2 * half[oth[1]]
             pdir[m, ax] = -sgn
-    emb = 0.5 * torch.randn(1, N, 32, generator=g)
+    emb = 0.5 * torch.randn(1, N, emb_dim, generator=g)
     color = torch.rand(1, N, 3, generator=g)
     conf = 0.1 + 0.9 * torch.rand(1, N, 1, generator=g)
     out = dict(xyz=xyz.float().contiguous(), embedding=emb, color=color, dir=pdir[None].float().contiguous(),
