@@ -254,6 +254,14 @@ int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts, const pnb_
                        const float* d_opacity /* [R,SR] or NULL */, const float* d_bg_T /* [R] or NULL */, int n_valid, int n_pairs,
                        float* d_emb, float* d_color, float* d_dir, float* d_conf, float* const* d_mlp_w, float* const* d_mlp_b, void* ws,
                        size_t ws_bytes, int flags, int* d_err, pnb_stream_t stream);
+/* Diagnostics / tests: device pointers of the forward recompute inside a workspace pnb_shade_backward ran in with the same n_valid,
+ * cap_samples and feat_dim; the buffers keep their contents after it returns.  out[10] receives, in this order:
+ *   H1, X3, H3, H4 (float, one row per valid pair: ld 256, 272 with H2 in columns 0..255, 256, 256), C1, C2, C3 (float [n_valid][128]):
+ *     the post-activations of the 7 LeakyReLU layers (block1.0, block1.2, block3.0, block3.2, color_branch.0 .2 .4); the backward takes
+ *     slope 1 where a value is > 0 and 0.01 elsewhere;
+ *   pair_off (uint32 [n_valid + 1], the first pair row of each valid sample), row_samp (int32 [n_pairs], valid-sample index of each
+ *     row), pidx (int32 [n_pairs], point index of each row). */
+int pnb_backward_tables(void* ws, size_t ws_bytes, int n_valid, int cap_samples, int feat_dim, void** out);
 
 #ifdef __cplusplus
 }

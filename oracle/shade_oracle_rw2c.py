@@ -12,16 +12,16 @@ Rw2c is handed to shade_oracle.shade unchanged.  Differentiable: autograd throug
 import torch
 import torch.nn.functional as F
 
-from .shade_oracle import LEAKY_SLOPE, _lin, fill_invalid, positional_encoding, w2pers  # noqa: F401  (fill_invalid: re-exported)
+from .shade_oracle import LEAKY_SLOPE, _act, _lin, fill_invalid, positional_encoding, w2pers  # noqa: F401  (fill_invalid: re-exported)
 from . import shade_oracle
 
 
 def shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w, vsize, bg_color,
-          dtype=torch.float32, agg_intrp_order=2):
+          dtype=torch.float32, agg_intrp_order=2, slopes=None):
     """The arguments and the returned dict of shade_oracle.shade; points["Rw2c"] is [3,3] or [N,3,3]."""
     if points["Rw2c"].dim() == 2:
         return shade_oracle.shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w, vsize, bg_color,
-                                  dtype=dtype, agg_intrp_order=agg_intrp_order)
+                                  dtype=dtype, agg_intrp_order=agg_intrp_order, slopes=slopes)
     assert agg_intrp_order in (1, 2)
     cv = lambda t: t.to(dtype)
     xyz = cv(points["xyz"]); emb = cv(points["embedding"][0]); col = cv(points["color"][0])
@@ -73,13 +73,13 @@ def shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w,
     d_pe = positional_encoding(d_flat, 5)
     f = s_emb.reshape(-1, s_emb.shape[-1])[pm]
     feat = torch.cat([f, positional_encoding(f, 3), d_pe], dim=-1)
-    act = lambda x: F.leaky_relu(x, LEAKY_SLOPE)
-    feat = act(_lin(act(_lin(feat, mlp, "block1.0")), mlp, "block1.2"))
+    act = lambda x, layer: _act(x, slopes, layer)
+    feat = act(_lin(act(_lin(feat, mlp, "block1.0"), 0), mlp, "block1.2"), 1)
     c_flat = s_col.reshape(-1, 3)[pm]
     dir_flat = rot_pair(s_dir.reshape(-1, 3)[pm])
     ov = ori_viewdirs[:, None, :].expand(-1, K, -1).reshape(-1, 3)[pm]
     feat = torch.cat([feat, c_flat, dir_flat - ov, torch.sum(dir_flat * ov, dim=-1, keepdim=True)], dim=-1)
-    feat = act(_lin(act(_lin(feat, mlp, "block3.0")), mlp, "block3.2"))
+    feat = act(_lin(act(_lin(feat, mlp, "block3.0"), 2), mlp, "block3.2"), 3)
     alpha = F.softplus(_lin(feat, mlp, "alpha_branch.0") - 1)
     n_pair = Rn * SR * K
     pm_idx = pm.nonzero()[:, 0]
@@ -92,9 +92,9 @@ def shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w,
     else:
         sigma = F.softplus(_lin(hbar, mlp, "alpha_branch.0") - 1)
     cin = torch.cat([hbar, pe_view], dim=-1)
-    x = act(_lin(cin, mlp, "color_branch.0"))
-    x = act(_lin(x, mlp, "color_branch.2"))
-    x = act(_lin(x, mlp, "color_branch.4"))
+    x = act(_lin(cin, mlp, "color_branch.0"), 4)
+    x = act(_lin(x, mlp, "color_branch.2"), 5)
+    x = act(_lin(x, mlp, "color_branch.4"), 6)
     rgb = torch.sigmoid(_lin(x, mlp, "color_branch.6")) * (1 + 2 * 0.001) - 0.001
     decoded = torch.cat([sigma, rgb], dim=-1)
     decoded = torch.where(sv[:, None], decoded, torch.zeros_like(decoded))

@@ -613,6 +613,18 @@ extern "C" size_t pnb_backward_bytes(int n_valid, int cap_samples, int feat_dim)
     return F > 0 ? carve(nullptr, 0, n_valid, cap_samples, F).bytes : 0;
 }
 
+// tests: device pointers of the recompute buffers inside a workspace pnb_shade_backward used with the same n_valid / cap_samples / F
+extern "C" int pnb_backward_tables(void* ws, size_t ws_bytes, int n_valid, int cap_samples, int feat_dim, void** out) {
+    const int F = feat_of(feat_dim);
+    PNB_REQUIRE(ws && out, PNB_ERR_INVALID, "pnb_backward_tables: null argument");
+    PNB_REQUIRE(F > 0, PNB_ERR_UNSUPPORTED, "pnb_backward_tables: point_features_dim %d unsupported", feat_dim);
+    const Layout L = carve(ws, ws_bytes, n_valid, cap_samples, F);
+    PNB_REQUIRE(L.bytes <= ws_bytes, PNB_ERR_WORKSPACE, "pnb_backward_tables: workspace %zu < required %zu", ws_bytes, L.bytes);
+    void* const t[10] = {L.H1, L.X3, L.H3, L.H4, L.C1, L.C2, L.C3, L.pair_off, L.row_samp, L.pidx};
+    for (int i = 0; i < 10; ++i) out[i] = t[i];
+    return PNB_OK;
+}
+
 // d_mlp_w[i] / d_mlp_b[i]: gradient accumulators in the layout of pnb_mlp_t (W^T [K_pad][N], bias [N]); the caller
 // zero-initialises them.  Point gradients are accumulated (atomicAdd) into d_emb/d_color/d_dir/d_conf (caller zeroes);
 // any of them may be NULL.  Upstream gradients: d_ray_color [R,3], d_opacity [R,SR], d_bg_T [R], each may be NULL (at least one is

@@ -255,8 +255,9 @@ static GridLayout carve_grid(void* buf, size_t cap, int N, const int32_t dim[3])
 
 using namespace pnb;
 
-extern "C" int pnb_version(void) { return 103; }   // 101: pnb_points_t.rw2c; 102: pnb_shade_backward takes d_opacity, d_bg_T;
-                                                   // 103: pnb_points_t / pnb_mlp_t.feat_dim (F = 32 | 63), F-sized *_bytes()
+extern "C" int pnb_version(void) { return 104; }   // 101: pnb_points_t.rw2c; 102: pnb_shade_backward takes d_opacity, d_bg_T;
+                                                   // 103: pnb_points_t / pnb_mlp_t.feat_dim (F = 32 | 63), F-sized *_bytes();
+                                                   // 104: pnb_backward_tables (test-only: the backward's recompute buffers)
 extern "C" const char* pnb_last_error(void) { return pnb::g_err; }
 extern "C" size_t pnb_struct_size(int which) {
     switch (which) {

@@ -86,7 +86,8 @@ def _rel(a, ref):
     return ((a.double() - ref).abs().max() / ref.abs().max().clamp_min(1e-30)).item()
 
 
-@pytest.mark.parametrize("M,N,K", [(300, 256, 288), (128, 128, 128), (1000, 256, 272), (77, 288, 256), (4096, 128, 128)])
+@pytest.mark.parametrize("M,N,K", [(300, 256, 288), (128, 128, 128), (1000, 256, 272), (77, 288, 256), (4096, 128, 128),
+                                   (1000, 256, 512)])   # F = 63: the 512-wide block1.0 recompute (its NT: 512 output columns)
 def test_gemm_tc_nn_nt(M, N, K):
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     X = torch.randn(M, K + 16, device="cuda", generator=g)[:, :K]                 # leading dimension != K
@@ -112,7 +113,27 @@ def test_gemm_tc_nn_nt(M, N, K):
         assert _rel(dX, refx * mask) < 2e-5
 
 
-@pytest.mark.parametrize("rows,Kin,Nout,splits", [(5000, 288, 256, 3), (130000, 256, 256, 64), (999, 128, 128, 2), (40000, 272, 256, 20)])
+@pytest.mark.parametrize("dact", [False, True])
+def test_gemm_tc_nt_partial_n_tile(dact):
+    """The F = 63 dX1 GEMM: 448 of the 512 columns of G1 (the 7F feature inputs rounded up to 16), a partial last N tile and a partial
+    last M tile; the columns beyond 448 are not written."""
+    M, Kin, Nout, ncol = 1000, 512, 256, 448
+    g = torch.Generator(device="cuda").manual_seed(448 + dact)
+    dZ = torch.randn(M, Nout, device="cuda", generator=g)
+    Wt = (0.1 * torch.randn(Kin, Nout, device="cuda", generator=g)).contiguous()   # W^T [Kin][Nout]
+    Y = torch.randn(M, Kin, device="cuda", generator=g) if dact else None
+    dX = _gemm_tc(dZ, Nout, 1, Wt, Nout, 1, M, ncol, Nout, Kin, dact=Y, ldd=Kin if dact else 0, dact_n=ncol if dact else 0)
+    ref = dZ.double() @ Wt[:ncol].double().t()
+    if dact:
+        ref = ref * torch.where(Y[:, :ncol] > 0, 1.0, 0.01).double()
+    assert _rel(dX[:, :ncol], ref) < 2e-5
+    assert torch.all(dX[:, ncol:] == 7.0)
+
+
+@pytest.mark.parametrize("rows,Kin,Nout,splits", [(5000, 288, 256, 3), (130000, 256, 256, 64), (999, 128, 128, 2), (40000, 272, 256, 20),
+                                                  # F = 63 block1.0 dW (Kin 512) at the backward's split counts: the 2-split
+                                                  # clamp, (rows + 2047) / 2048, and the 64-split cap
+                                                  (3000, 512, 256, 2), (40000, 512, 256, 20), (130000, 512, 256, 64)])
 def test_gemm_tc_tn_splitk_accumulate(rows, Kin, Nout, splits):
     """dWt[Kin x Nout] += X^T dZ: both operands transposed on the way into shared memory, deterministic split-K, accumulation."""
     g = torch.Generator(device="cuda").manual_seed(rows)
