@@ -261,11 +261,13 @@ __global__ void __launch_bounds__(256) k_pack_block1_f63(const float* __restrict
 }
 
 // Weight ring of the pair and colour kernels.  Consumption m (one K = 16 step, counted over the CTA's whole tile sequence) uses
-// stage m % NSTAGE.  Thread 0 issues the loads; every consumer warp releases a stage once the wgmma group that read it has
-// retired, and thread 0 then refills the stage with consumption m + NSTAGE.  The weights do not depend on the tile, so the ring
-// runs ahead across tile boundaries.
+// stage m % NSTAGE.  One producer thread, outside the consumer warpgroups, runs the whole sequence: it waits until the 8 consumer
+// warps have released the stage's previous consumption and refills it.  A consumer warp only waits for `full` and releases a stage
+// once the wgmma group that read it has retired (a predicated arrive of lane 0): nothing divergent sits between its wgmma, so ptxas
+// keeps them asynchronous.  The weights do not depend on the tile, so the ring runs ahead across tile boundaries.
 template <int NSTAGE, int STEP, class ImgOf>
 struct Ring {
+    static constexpr uint32_t CONSUMER_WARPS = 8;         // arrivals that empty a stage
     unsigned char (*buf)[STEP];
     uint64_t* full;
     uint64_t* empty;
@@ -273,28 +275,24 @@ struct Ring {
     uint32_t total;
     ImgOf img_of;
     int* err;
-    __device__ __forceinline__ void load(uint32_t m) {
-        const uint32_t s = m % NSTAGE;
-        mbar_arrive_expect_tx(&full[s], STEP);
-        bulk_g2s(buf[s], src + (size_t)img_of(m) * STEP, STEP, &full[s]);
+    __device__ __forceinline__ void init() {              // one thread, before the CTA-wide barrier that publishes the ring
+        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMER_WARPS); }
     }
-    __device__ __forceinline__ void prologue() {          // thread 0
-        for (uint32_t m = 0; m < total && m < (uint32_t)NSTAGE; ++m) load(m);
+    // the producer thread; after a failed (timed-out) wait it stops refilling and the consumers' waits report their own time-out
+    __device__ __forceinline__ void produce() {
+#pragma unroll 1
+        for (uint32_t m = 0; m < total; ++m) {
+            const uint32_t s = m % NSTAGE;
+            if (m >= (uint32_t)NSTAGE && !mbar_wait(&empty[s], (m / NSTAGE - 1u) & 1u, err, 92)) return;
+            mbar_arrive_expect_tx(&full[s], STEP);
+            bulk_g2s(buf[s], src + (size_t)img_of(m) * STEP, STEP, &full[s]);
+        }
     }
     // after a failed (timed-out) wait `ok` stays false: later waits are skipped, every barrier is still reached, the error flag is set
     __device__ __forceinline__ bool acquire(uint32_t m, bool ok) {
         return ok && mbar_wait(&full[m % NSTAGE], (m / NSTAGE) & 1u, err, 91);
     }
-    __device__ __forceinline__ bool release(uint32_t m, bool ok) {
-        __syncwarp();
-        if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[m % NSTAGE]);
-        if (threadIdx.x == 0 && m + NSTAGE < total) {
-            ok = ok && mbar_wait(&empty[m % NSTAGE], (m / NSTAGE) & 1u, err, 92);
-            if (ok) load(m + NSTAGE);
-        }
-        __syncwarp();                                     // the warp reconverges before the next wgmma (.sync.aligned)
-        return ok;
-    }
+    __device__ __forceinline__ void release(uint32_t m) { mbar_arrive_if(&empty[m % NSTAGE], (threadIdx.x & 31) == 0); }
 };
 
 // ------------------------------------------------------------------------------------------ row packing
@@ -515,8 +513,9 @@ __global__ void __launch_bounds__(256) k_point_pre(const float* __restrict__ emb
 
 // =====================================================================================================================
 // k_shade_wg: the pair MLPs of the packed 128-row tiles (a tile is four 32-row quadrants, each holding whole samples back to back,
-// only their valid neighbours: 99 % of the rows carry a pair on the lego frame).  One persistent CTA per SM, 256 threads = two
-// consumer warpgroups; warpgroup c owns tile rows 64c .. 64c+63 of every layer (wgmma M = 64, N = 256: a 128-register fp32
+// only their valid neighbours: 99 % of the rows carry a pair on the lego frame).  One persistent CTA per SM, 384 threads = two
+// consumer warpgroups + a producer warpgroup (one thread of warp 8 runs the weight ring; it hands its registers to the consumers
+// with setmaxnreg); warpgroup c < 2 owns tile rows 64c .. 64c+63 of every layer (wgmma M = 64, N = 256: a 128-register fp32
 // accumulator per thread).  Per tile:
 //   build     two threads per row (operand columns 0..151 | 152..287 of block1.0; FROZEN: one thread per row, PE5(dists) only) write
 //             the layer-1 operand (bf16 hi / lo, core-matrix layout) and the block3 extras operand into shared memory
@@ -527,7 +526,13 @@ __global__ void __launch_bounds__(256) k_point_pre(const float* __restrict__ emb
 //             sample with lane = row (segmented warp scan; its addition order depends on the neighbour count only, so a ray's colour
 //             does not depend on which rays share the call): h-bar + sigma
 namespace hw {
-constexpr int NTHR = 256;
+constexpr int NTHR = 256;                 // the two consumer warpgroups
+constexpr int NTHR_CTA = NTHR + 128;      // + warpgroup 2: the weight-ring producer (one thread of warp 8)
+// setmaxnreg budgets: the launch gives 168 registers per thread (65,536 / 384, rounded down to 8); the CTA's 64,512 are
+// redistributed as 2 x 128 x REGS_CONSUMER + 128 x REGS_PRODUCER.  At 232 consumer registers the frozen per-point-frame
+// instantiations spill; the producer loop fits in 24.
+constexpr uint32_t REGS_CONSUMER = 240, REGS_PRODUCER = 24;
+static_assert(2 * 128 * REGS_CONSUMER + 128 * REGS_PRODUCER <= 168 * NTHR_CTA, "register budgets exceed the launch allocation");
 constexpr int NSTAGE = 4;
 constexpr int YLD = 260;                  // fp32 row stride of the last-epilogue buffer: lane = row float4 reads are conflict-free
 // first K step of the frozen layer 1: the distance PE (F = 32: operand columns 224..287 of block1.0; F = 63: 0..63, tc::w1_row_f63)
@@ -566,7 +571,7 @@ __device__ __forceinline__ uint32_t step_image(uint32_t j, bool frozen) {
 // retires (both warpgroups), the builders write the second half over it and the accumulator carries on.  FROZEN does not read the
 // features: only its layer-1 weight images differ.
 template <bool FROZEN, bool O1, bool PP, int F>
-__global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
+__global__ void __launch_bounds__(hw::NTHR_CTA, 1) k_shade_wg(ShadeTcParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     hw::Smem& sm = *reinterpret_cast<hw::Smem*>(smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u));
@@ -579,16 +584,21 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
     const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     constexpr bool SPLIT = F != PNB_FEAT && !FROZEN;              // layer 1 in two halves
     constexpr uint32_t ST = (uint32_t)(hw::steps_of(0, FROZEN, F) + 16 + 17 + 16);
+    auto img_of = [](uint32_t m) { return hw::step_image<F>(m % ST, FROZEN); };
+    Ring<hw::NSTAGE, STEP, decltype(img_of)> ring{sm.b, sm.bar_full, sm.bar_empty, p.wimg, (uint32_t)my_tiles * ST, img_of, p.err};
 
     if (tid == 0) {
-        for (int s = 0; s < hw::NSTAGE; ++s) { mbar_init(&sm.bar_full[s], 1); mbar_init(&sm.bar_empty[s], hw::NTHR / 32); }
+        ring.init();
         mbar_fence_init();
         if (blockIdx.x == 0 && q.counters[PNB_QC_N_VALID] > p.hbar_cap) atomicExch(p.err, 9);
     }
     __syncthreads();
-    auto img_of = [](uint32_t m) { return hw::step_image<F>(m % ST, FROZEN); };
-    Ring<hw::NSTAGE, STEP, decltype(img_of)> ring{sm.b, sm.bar_full, sm.bar_empty, p.wimg, (uint32_t)my_tiles * ST, img_of, p.err};
-    if (tid == 0) ring.prologue();
+    if (wgi == 2) {                                              // producer warpgroup
+        setmaxnreg_dec<hw::REGS_PRODUCER>();
+        if (tid == hw::NTHR) ring.produce();
+        return;
+    }
+    setmaxnreg_inc<hw::REGS_CONSUMER>();
 
     const uint32_t a_hi0 = smem_u32(sm.a_hi) + (uint32_t)wgi * 4096u, a_lo0 = smem_u32(sm.a_lo) + (uint32_t)wgi * 4096u;
     const uint32_t xe_hi0 = smem_u32(sm.xe_hi) + (uint32_t)wgi * 2048u, xe_lo0 = smem_u32(sm.xe_lo) + (uint32_t)wgi * 2048u;
@@ -661,11 +671,11 @@ __global__ void __launch_bounds__(hw::NTHR, 1) k_shade_wg(ShadeTcParams p) {
                 mma_n256(acc, ah, bl, 1u);
                 wg::commit();
                 wg::wait<1>();
-                if (kk > 0) ok = ring.release(m - 1, ok);
+                if (kk > 0) ring.release(m - 1);
             }
             wg::wait<0>();
             pin<128>(acc);
-            ok = ring.release(m - 1, ok);
+            ring.release(m - 1);
             if (l == 3) break;
             // epilogue: + bias (FROZEN layer 1: + pre[point of the row], which includes the bias), LeakyReLU, bf16 hi / lo split
             const float* bias = p.bias[l];
@@ -767,10 +777,12 @@ struct ColorTcParams {
 // k_color_wg: the colour branch per 128 consecutive valid samples.  The pair kernel writes h-bar already split into bf16 hi / lo
 // and laid out as this kernel's A-operand blocks (per 128 samples 8 K blocks x {hi, lo} x [128 x 32], one contiguous 128 KB region),
 // so the layer-1 operand is one bulk copy per tile; threads 0-127 add the PE(view) K block.  Two consumer warpgroups of 64 rows
-// (wgmma N = 128), the same weight ring and in-place operand epilogues as k_shade_wg; the last layer (128 -> 3 + sigmoid) runs on
-// CUDA cores straight from the accumulator fragments.
+// (wgmma N = 128), the same producer warpgroup, weight ring and in-place operand epilogues as k_shade_wg; the last layer
+// (128 -> 3 + sigmoid) runs on CUDA cores straight from the accumulator fragments.
 namespace hcw {
-constexpr int NTHR = 256, NSTAGE = 4;
+constexpr int NTHR = 256, NSTAGE = 4;         // consumer threads
+constexpr int NTHR_CTA = NTHR + 128;          // + the producer warpgroup, as in k_shade_wg
+constexpr uint32_t REGS_CONSUMER = hw::REGS_CONSUMER, REGS_PRODUCER = hw::REGS_PRODUCER;
 constexpr int BLK = 128 * 64;                 // [128 x 32] bf16 block
 constexpr int STEP = 2 * 128 * 32;            // hi + lo image ([128 x 16] bf16 each) of one K = 16 step
 constexpr int TILE_BYTES = 8 * 2 * BLK;       // h-bar operand of one tile in global memory
@@ -784,7 +796,7 @@ struct Smem {
 
 // PP: per-point frames (the view direction in the frame of each sample's slot-0 point)
 template <bool PP>
-__global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
+__global__ void __launch_bounds__(hcw::NTHR_CTA, 1) k_color_wg(ColorTcParams p) {
     using namespace hcw;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     Smem& sm = *reinterpret_cast<Smem*>(smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u));
@@ -794,15 +806,20 @@ __global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
     const int n_tiles = (n_valid + 127) / 128;
     const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
+    auto img_of = [](uint32_t m) { return m % ST; };
+    Ring<NSTAGE, STEP, decltype(img_of)> ring{sm.b, sm.bar_full, sm.bar_empty, p.wimg, (uint32_t)my_tiles * ST, img_of, p.err};
     if (tid == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&sm.bar_full[s], 1); mbar_init(&sm.bar_empty[s], NTHR / 32); }
+        ring.init();
         mbar_init(&sm.bar_a, 1);
         mbar_fence_init();
     }
     __syncthreads();
-    auto img_of = [](uint32_t m) { return m % ST; };
-    Ring<NSTAGE, STEP, decltype(img_of)> ring{sm.b, sm.bar_full, sm.bar_empty, p.wimg, (uint32_t)my_tiles * ST, img_of, p.err};
-    if (tid == 0) ring.prologue();
+    if (wgi == 2) {                                              // producer warpgroup
+        setmaxnreg_dec<REGS_PRODUCER>();
+        if (tid == NTHR) ring.produce();
+        return;
+    }
+    setmaxnreg_inc<REGS_CONSUMER>();
 
     const uint32_t a0 = smem_u32(sm.a[0][0]) + (uint32_t)wgi * 4096u, b0 = smem_u32(sm.b[0]);
     const int r0 = 64 * wgi + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
@@ -862,11 +879,11 @@ __global__ void __launch_bounds__(hcw::NTHR, 1) k_color_wg(ColorTcParams p) {
                 mma_n128(acc, ah, bl, 1u);
                 wg::commit();
                 wg::wait<1>();
-                if (kk > 0) ok = ring.release(m - 1, ok);
+                if (kk > 0) ring.release(m - 1);
             }
             wg::wait<0>();
             pin<64>(acc);
-            ok = ring.release(m - 1, ok);
+            ring.release(m - 1);
             const float* bias = p.bias[l];
             if (l < 2) {
 #pragma unroll
@@ -1082,7 +1099,7 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
                                           : (pp ? k_shade_wg<true, false, true, PNB_FEAT_DTU> : k_shade_wg<true, false, false, PNB_FEAT_DTU>))
                                     : (o1 ? (pp ? k_shade_wg<false, true, true, PNB_FEAT_DTU> : k_shade_wg<false, true, false, PNB_FEAT_DTU>)
                                           : (pp ? k_shade_wg<false, false, true, PNB_FEAT_DTU> : k_shade_wg<false, false, false, PNB_FEAT_DTU>)));
-        kern<<<n_cta, hw::NTHR, smem_pair, stream>>>(p);
+        kern<<<n_cta, hw::NTHR_CTA, smem_pair, stream>>>(p);
     }
     if (flags & PNB_TC_COLOR) {
         ColorTcParams ct;
@@ -1091,8 +1108,8 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
         ct.w3t = mlp->w[8]; ct.b3 = mlp->b[8];
         ct.hbar = w.hbar; ct.sigma = w.sigma; ct.hbar_cap = max_valid_samples; ct.sigma_rgb = (float4*)d_sigma_rgb; ct.err = d_err;
         ct.pts = *pts;
-        if (pts->rw2c) k_color_wg<true><<<n_cta, hcw::NTHR, smem_color, stream>>>(ct);
-        else k_color_wg<false><<<n_cta, hcw::NTHR, smem_color, stream>>>(ct);
+        if (pts->rw2c) k_color_wg<true><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
+        else k_color_wg<false><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
     }
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
