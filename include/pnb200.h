@@ -150,8 +150,8 @@ typedef struct {
 
 int pnb_version(void);
 const char* pnb_last_error(void);
-/* sizeof() of the POD structs above as the library was compiled (0 grid, 1 query, 2 shade_opts, 3 mlp,
- * 4 points) -- lets a foreign-language binding verify its mirror of the layout. */
+/* sizeof() of the POD structs as the library was compiled (0 grid, 1 query, 2 shade_opts, 3 mlp,
+ * 4 points, 5 frustum) -- lets a foreign-language binding verify its mirror of the layout. */
 size_t pnb_struct_size(int which);
 
 /* ---- voxel grid ---- */
@@ -262,6 +262,65 @@ int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts, const pnb_
  *   pair_off (uint32 [n_valid + 1], the first pair row of each valid sample), row_samp (int32 [n_pairs], valid-sample index of each
  *     row), pidx (int32 [n_pairs], point index of each row). */
 int pnb_backward_tables(void* ws, size_t ws_bytes, int n_valid, int cap_samples, int feat_dim, void** out);
+
+/* ---- perspective-frustum neighbour query (wcoord_query 0, NN 2) ----
+ * Replaces models/neural_points/query_point_indices.py:263-770 (get_occ_vox, near_vox_full, insert_vox_points,
+ * query_neigh_along_ray_layered and their host glue) for the drop-in pointnerf_b200.query_point_indices.  Canonical serial semantics
+ * and the reference's quirks: DESIGN.md §5 F1-F9.  The build depends on the points (in perspective coordinates x/z, y/z, z) and the
+ * grid only, never on the rays, so one build serves every ray chunk of a view. */
+enum {                             /* counters written by pnb_frustum_build (device int32[16]) */
+    PNB_FB_N_VOX = 0,              /* voxels holding >= 1 point (truncated coordinates) */
+    PNB_FB_MAX_PTS = 1,            /* max points in one voxel (before the P cap) */
+    PNB_FB_OVERFLOW_P = 2,         /* voxels with > P points (reference: curand reservoir; here: first P by index) */
+    PNB_FB_N_INSERT = 3,           /* points bucketed by truncated coordinates */
+    PNB_FB_N_OCC = 4,              /* points inside the grid by floored coordinates */
+    PNB_FB_MAX_COL_VOX = 5,        /* max occupied voxels in one column */
+    PNB_FB_OVERFLOW_O = 6,         /* 1 if MAX_COL_VOX > max_o (or > 127, the int8 numbering): the reference wraps or overruns */
+    PNB_FB_MAX_COL_SAMPLES = 7,    /* max dilated voxels in one column before the SR cap */
+    PNB_FB_N_COL_CAPPED = 8        /* columns with more than SR dilated voxels (only the first SR are sampled) */
+};
+enum {                             /* counters written by pnb_frustum_query (device int32[16] in its workspace) */
+    PNB_FQ_R2 = 0,                 /* rays with ray_mask 1 (R') */
+    PNB_FQ_N_BAD_PIXEL = 1         /* pixels outside the grid (ray_mask 0; the reference reads out of bounds) */
+};
+typedef struct {
+    float lo[3];            /* ranges[0:3] of get_hyperparameters: x/z, y/z of the image corner, near */
+    float svs[3];           /* scaled voxel size (vsize * vscale) */
+    float rvs[2];           /* pixel size: svs / vscale (x, y) */
+    int32_t dim[3];         /* scaled_vdim */
+    int32_t vscale[2];
+    int32_t kernel_size[3];
+    int32_t query_size[3];
+    int32_t SR, K, P, n_points, max_o;
+    uint32_t n_words;       /* words of one volume bitmask */
+    uint32_t* pt_bits;      /* voxels holding a point by truncated coordinates (the CSR's voxels) */
+    uint32_t* occ_bits;     /* voxels holding a point by floored coordinates (the voxels the query searches) */
+    uint32_t* word_rank;    /* exclusive prefix of popc(pt_bits[w]) */
+    uint32_t* vox_start;    /* CSR offsets into spts */
+    float* spts;            /* float4 (x, y, z, bitcast point index), voxel-major, ascending index */
+    int16_t* col_list;      /* [dim0*dim1, SR] first SR depth ids of each column's dilated occupancy, -1 padded */
+    int32_t* col_far;       /* [dim0*dim1] last dilated depth id of each column (-1: none) */
+    int32_t* counters;      /* device int32[16], see PNB_FB_* */
+} pnb_frustum_t;
+
+size_t pnb_frustum_bytes(int N, const int32_t dim[3], int SR);
+/* NN != 2, inverse != 0, B != 1, K > PNB_MAX_K, SR > PNB_MAX_SR, or a query_size that does not cover the kernel_size search:
+ * PNB_ERR_UNSUPPORTED.  max_o <= 0: derived (the reference's default).  h_counters (optional) synchronises. */
+int pnb_frustum_build(pnb_frustum_t* fr, void* buf, size_t buf_bytes, const float* d_xyz_pers, int N, int B, const float lo[3],
+                      const float svs[3], const int32_t dim[3], const int32_t vscale[3], const int32_t kernel_size[3],
+                      const int32_t query_size[3], int SR, int K, int P, int max_o, int NN, int inverse, pnb_stream_t stream,
+                      int32_t* h_counters);
+/* Ray mask of R pixels (int32 [R,2], (x, y)) and the compaction scan; R' lands in counters[PNB_FQ_R2] of the workspace and, with
+ * h_counters (which synchronises), on the host. */
+size_t pnb_frustum_query_bytes(int R);
+int pnb_frustum_query(const pnb_frustum_t* fr, const int32_t* d_pixel_idx, int R, void* ws, size_t ws_bytes, int8_t* d_ray_mask,
+                      pnb_stream_t stream, int32_t* h_counters);
+/* Dense reference layout for the R2 = R' rays of a pnb_frustum_query in the same workspace: pixel_idx_cur [R2,2],
+ * sample_pidx [R2,SR,K] (-1 padded), sample_loc [R2,SR,3] (perspective; written for every slot).  radius_limit2 / depth_limit2: the
+ * squared limits as the reference passes them (np.float32(limit ** 2)); 0 = no limit. */
+int pnb_frustum_export(const pnb_frustum_t* fr, const int32_t* d_pixel_idx, int R, const void* ws, size_t ws_bytes,
+                       const int8_t* d_ray_mask, int R2, float radius_limit2, float depth_limit2, int32_t* d_pixel_idx_cur,
+                       int32_t* d_sample_pidx, float* d_sample_loc, pnb_stream_t stream);
 
 #ifdef __cplusplus
 }

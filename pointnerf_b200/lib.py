@@ -51,15 +51,26 @@ class Points(C.Structure):
                 ("conf", C.c_void_p), ("N", C.c_int32), ("rw2c", C.c_void_p), ("feat_dim", C.c_int32)]
 
 
+class Frustum(C.Structure):
+    _fields_ = [("lo", C.c_float * 3), ("svs", C.c_float * 3), ("rvs", C.c_float * 2), ("dim", C.c_int32 * 3),
+                ("vscale", C.c_int32 * 2), ("kernel_size", C.c_int32 * 3), ("query_size", C.c_int32 * 3), ("SR", C.c_int32),
+                ("K", C.c_int32), ("P", C.c_int32), ("n_points", C.c_int32), ("max_o", C.c_int32), ("n_words", C.c_uint32),
+                ("pt_bits", C.c_void_p), ("occ_bits", C.c_void_p), ("word_rank", C.c_void_p), ("vox_start", C.c_void_p),
+                ("spts", C.c_void_p), ("col_list", C.c_void_p), ("col_far", C.c_void_p), ("counters", C.c_void_p)]
+
+
 GC = dict(n_occ=0, max_pts=1, overflow_o=2, overflow_p=3, n_inrange=4, slot0_cell=5, first_pt=6)
 QC = dict(n_cand=0, n_valid=1, n_pairs=2, R1=3, R2=4, overflow=5)
+FB = dict(n_vox=0, max_pts=1, overflow_p=2, n_insert=3, n_occ=4, max_col_vox=5, overflow_o=6, max_col_samples=7, n_col_capped=8)
+FQ = dict(R2=0, n_bad_pixel=1)
 
 # every symbol include/pnb200.h declares (tests check that the .so exports all of them)
 SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes", "pnb_grid_build", "pnb_query_bytes", "pnb_query",
            "pnb_query_export", "pnb_shade_bytes", "pnb_shade_forward", "pnb_composite_forward",
            "pnb_mlp_pack_bytes", "pnb_mlp_pack", "pnb_point_pre_bytes", "pnb_point_pre", "pnb_shade_tc_bytes", "pnb_shade_forward_tc",
            "pnb_shade_tc_tables", "pnb_backward_bytes", "pnb_shade_backward", "pnb_backward_tables", "pnb_aux_outputs",
-           "pnb_aux_conf_backward"]
+           "pnb_aux_conf_backward", "pnb_frustum_bytes", "pnb_frustum_build", "pnb_frustum_query_bytes", "pnb_frustum_query",
+           "pnb_frustum_export"]
 # test-only library (csrc/selftest/pnb200_selftest.h)
 SELFTEST_LIB_PATH = os.path.join(_HERE, "csrc", "libpnb200_selftest.so")
 SELFTEST_SYMBOLS = ["pnb_selftest_last_error", "pnb_umma_selftest", "pnb_umma_selftest2", "pnb_gemm_tc_test"]
@@ -84,7 +95,7 @@ def load():
     lib.pnb_last_error.restype = C.c_char_p
     lib.pnb_struct_size.restype = C.c_size_t
     lib.pnb_struct_size.argtypes = [C.c_int]
-    for which, ty in enumerate((Grid, Query, ShadeOpts, Mlp, Points)):
+    for which, ty in enumerate((Grid, Query, ShadeOpts, Mlp, Points, Frustum)):
         if lib.pnb_struct_size(which) != C.sizeof(ty):
             raise PnbError("ABI mismatch: struct %s is %d bytes in libpnb200.so, %d in the binding"
                            % (ty.__name__, lib.pnb_struct_size(which), C.sizeof(ty)))
@@ -141,6 +152,21 @@ def load():
                                        C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p]
     lib.pnb_backward_tables.restype = C.c_int
     lib.pnb_backward_tables.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
+    lib.pnb_frustum_bytes.restype = C.c_size_t
+    lib.pnb_frustum_bytes.argtypes = [C.c_int, C.POINTER(C.c_int32), C.c_int]
+    lib.pnb_frustum_build.restype = C.c_int
+    lib.pnb_frustum_build.argtypes = [C.POINTER(Frustum), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float),
+                                      C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                      C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                      C.POINTER(C.c_int32)]
+    lib.pnb_frustum_query_bytes.restype = C.c_size_t
+    lib.pnb_frustum_query_bytes.argtypes = [C.c_int]
+    lib.pnb_frustum_query.restype = C.c_int
+    lib.pnb_frustum_query.argtypes = [C.POINTER(Frustum), C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                      C.POINTER(C.c_int32)]
+    lib.pnb_frustum_export.restype = C.c_int
+    lib.pnb_frustum_export.argtypes = [C.POINTER(Frustum), C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_float,
+                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = lib
     return lib
 

@@ -91,6 +91,10 @@ def check_opt(opt):
         raise NotImplementedError("pnb200: agg_axis_weight must be None or 1 1 1")
     if getattr(opt, "prob", 0) not in (0, 1):
         raise NotImplementedError("pnb200: opt.prob must be 0 or 1")
+    if int(getattr(opt, "wcoord_query", -1)) == 0:
+        # the perspective-frustum query has its own drop-in (pointnerf_b200.query_point_indices); the fused module only runs the world grid
+        raise NotImplementedError("pnb200: wcoord_query=0 (perspective-frustum query) is not part of the fused module; "
+                                  "use pointnerf_b200.query_point_indices as the reference's querier")
     if float(getattr(opt, "xyz_grad", 0) or 0) > 0:
         # the fused backward produces no d/d(xyz) (every shipped script has xyz_grad = 0): refuse instead of silently freezing xyz
         raise NotImplementedError("pnb200: xyz_grad > 0 (point positions as trainable parameters) is outside the implemented hot path")

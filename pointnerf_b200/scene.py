@@ -145,3 +145,81 @@ def ranges_for(cfg: SceneConfig):
         e = cfg.R_s + 0.1
         return (-e, -e, -e, e, e, e)
     return (-10.0,) * 3 + (10.0,) * 3
+
+
+# ---- DTU-like scenes of the perspective-frustum query (wcoord_query 0, NN 2; the DTU scripts' query options) ----
+@dataclass
+class FrustumConfig:
+    name: str
+    N: int = 30_000
+    H: int = 120
+    W: int = 160
+    focal: float = 200.0
+    near: float = 2.0
+    far: float = 4.725
+    z_depth_dim: int = 400
+    vscale: tuple = (2, 2, 1)
+    kernel_size: tuple = (3, 3, 3)
+    query_size: tuple = (3, 3, 3)
+    SR: int = 40
+    K: int = 8
+    P: int = 20
+    radius_limit_scale: float = 0.0
+    depth_limit_scale: float = 0.0
+    seed: int = 4321
+
+
+FRUSTUM_CONFIGS = {
+    "dtu_surface": FrustumConfig("dtu_surface"),
+    # non-zero limits: the radius / depth branch of the layered search
+    "dtu_surface_limits": FrustumConfig("dtu_surface_limits", radius_limit_scale=1.5, depth_limit_scale=1.2),
+}
+
+
+def make_frustum_scene(cfg: FrustumConfig):
+    """A bumpy surface about 2.5 units in front of a pinhole camera, plus 2 % of points scattered around the frustum (some of them
+    within one voxel outside the grid, where truncation and floor differ).  Returns numpy xyz_cam [N,3], pers [N,3] (x/z, y/z, z as
+    NeuralPoints.w2pers forms it), the world frame (camrotc2w [3,3], campos [3], xyz_w [N,3]), intrinsic [3,3] and the full-frame
+    pixel_idx [H*W,2] (x, y; y outer)."""
+    g = np.random.RandomState(cfg.seed)
+    n_out = cfg.N // 50
+    n_surf = cfg.N - n_out
+    u = g.uniform(-0.45, 0.45, n_surf) * cfg.W / cfg.focal
+    v = g.uniform(-0.45, 0.45, n_surf) * cfg.H / cfg.focal
+    z = 2.5 + 0.25 * np.sin(3.0 * u) * np.cos(2.0 * v) + 0.6 * (u * u + v * v) + 0.004 * g.randn(n_surf)
+    surf = np.stack([u * z, v * z, z], -1)
+    xr, yr = 0.5 * cfg.W / cfg.focal + 0.01, 0.5 * cfg.H / cfg.focal + 0.01
+    zo = g.uniform(cfg.near - 0.02, cfg.far + 0.02, n_out)
+    out = np.stack([g.uniform(-xr, xr, n_out) * zo, g.uniform(-yr, yr, n_out) * zo, zo], -1)
+    xyz_cam = np.concatenate([surf, out])[g.permutation(cfg.N)].astype(np.float32)
+    pers = np.stack([xyz_cam[:, 0] / xyz_cam[:, 2], xyz_cam[:, 1] / xyz_cam[:, 2], xyz_cam[:, 2]], -1).astype(np.float32)
+    a = 0.3
+    camrotc2w = np.array([[math.cos(a), 0.0, math.sin(a)], [0.0, 1.0, 0.0], [-math.sin(a), 0.0, math.cos(a)]], np.float32)
+    campos = np.array([0.2, -0.1, -0.3], np.float32)
+    xyz_w = (xyz_cam @ camrotc2w.T + campos).astype(np.float32)
+    intrinsic = np.array([[cfg.focal, 0, cfg.W / 2], [0, cfg.focal, cfg.H / 2], [0, 0, 1]], np.float32)
+    px, py = np.meshgrid(np.arange(cfg.W), np.arange(cfg.H))
+    pixel_idx = np.stack((px, py), -1).reshape(-1, 2).astype(np.int32)
+    return dict(xyz_cam=xyz_cam, pers=pers, camrotc2w=camrotc2w, campos=campos, xyz_w=xyz_w, intrinsic=intrinsic, pixel_idx=pixel_idx)
+
+
+def frustum_opt(cfg: FrustumConfig, is_train=False, **over):
+    """The querier options of the DTU scripts (dev_scripts/dtu_test_inf/inftest_scan*.sh) for one FrustumConfig."""
+    from types import SimpleNamespace
+    o = SimpleNamespace(inverse=0, NN=2, K=cfg.K, SR=cfg.SR, P=cfg.P, max_o=None, z_depth_dim=cfg.z_depth_dim, vscale=list(cfg.vscale),
+                        kernel_size=list(cfg.kernel_size), query_size=list(cfg.query_size), radius_limit_scale=cfg.radius_limit_scale,
+                        depth_limit_scale=cfg.depth_limit_scale, gpu_maxthr=1024, is_train=is_train, shpnt_jitter="uniform",
+                        wcoord_query=0)
+    for k, v in over.items():
+        setattr(o, k, v)
+    return o
+
+
+def make_frustum_points(cfg: FrustumConfig, s, emb_dim=63):
+    """Seeded neural-point attributes for a frustum scene (world xyz from make_frustum_scene): the dict the shading oracles take."""
+    g = torch.Generator().manual_seed(cfg.seed + 1)
+    N = s["xyz_w"].shape[0]
+    d = torch.randn(N, 3, generator=g)
+    return dict(xyz=torch.from_numpy(s["xyz_w"]), embedding=0.5 * torch.randn(1, N, emb_dim, generator=g),
+                color=torch.rand(1, N, 3, generator=g), dir=(d / d.norm(dim=-1, keepdim=True))[None],
+                conf=0.1 + 0.9 * torch.rand(1, N, 1, generator=g), Rw2c=torch.eye(3))
