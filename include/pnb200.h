@@ -230,6 +230,10 @@ int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pts, const pn
  * (vorder uint32[n_valid], vcntp uint8[n_valid], quad_first uint32[n_quads + 1], pack_cnt int32[1] = n_quads). */
 int pnb_shade_tc_tables(void* ws, size_t ws_bytes, int max_valid_samples, void** vorder, void** vcntp, void** quad_first,
                         void** pack_cnt);
+/* Tests: device pointers of the pair kernel's products inside the same workspace.  hbar: the K-reduced feature of every valid
+ * sample as k_color_wg's A operand, per 128 valid samples (vi >> 7) 8 blocks of 16 KB (bf16 hi 8 KB, then lo 8 KB, [128 x 32] in the
+ * core-matrix layout of wgmma.cuh), one per 32 channels; sigma: float[n_valid], by valid-sample index. */
+int pnb_shade_tc_buffers(void* ws, size_t ws_bytes, int max_valid_samples, void** hbar, void** sigma);
 
 /* ---- backward (per-scene optimisation batches) ----
  * Replaces loss.backward() through the reference's eager autograd graph

@@ -116,7 +116,7 @@ def shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w,
     acc_T = torch.cat([torch.ones(Rn, 1, dtype=dtype), acc[:, :-1]], dim=-1)
     blend_weight = (opacity * acc_T)[..., None]
     ray_color = torch.sum(decoded[..., 1:4] * blend_weight, dim=-2) + bg_color.view(1, 3) * bg_T
-    return dict(decoded=decoded, ray_valid=ray_valid, weight=weight, conf_coefficient=conf_coefficient,
+    return dict(decoded=decoded, ray_valid=ray_valid, weight=weight, conf_coefficient=conf_coefficient, hbar=hbar,
                 ray_dist=ray_dist, opacity=opacity, acc_T=acc_T, blend_weight=blend_weight, bg_T=bg_T,
                 ray_color=ray_color, sample_loc=sample_loc,
                 queried_shading=torch.logical_not(torch.any(ray_valid, dim=-1, keepdim=True)).repeat(1, 3).to(dtype))

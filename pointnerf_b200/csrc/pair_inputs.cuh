@@ -35,11 +35,15 @@ __device__ __forceinline__ void w2pers(const pnb_shade_opts_t& o, float px, floa
     rot3T(o.camrotc2w, px - o.campos[0], py - o.campos[1], pz - o.campos[2], xc, yc, zc);
     xp = xc / zc; yp = yc / zc; zp = zc;
 }
-// camera-space depth of a world position (z of w2pers)
+// camera-space depth of a world position (z of w2pers), rounded as the reference's torch.sum(shift[..., :, None] * camrotc2w, -2):
+// each product rounded, then summed in order, never contracted to FMAs.  The ray distances are differences of these depths, and the
+// raydist_mode_unit test (> 2 vsize_z) decides on their last bit where consecutive samples lie exactly 2 vsize_z apart in depth; there,
+// one rounding apart replaces a step by vsize_z and moves the ray's colour by a few 1e-2 (rotated cameras; the identity's products are
+// exact, so there any order gives the same bits).
 __device__ __forceinline__ float cam_depth(const pnb_shade_opts_t& o, float3 x) {
-    float xc, yc, zc;
-    rot3T(o.camrotc2w, x.x - o.campos[0], x.y - o.campos[1], x.z - o.campos[2], xc, yc, zc);
-    return zc;
+    const float* M = o.camrotc2w;
+    const float sx = x.x - o.campos[0], sy = x.y - o.campos[1], sz = x.z - o.campos[2];
+    return __fadd_rn(__fadd_rn(__fmul_rn(sx, M[2]), __fmul_rn(sy, M[5])), __fmul_rn(sz, M[8]));
 }
 
 // ------------------------------------------------------------------------------------------ samples

@@ -1033,6 +1033,14 @@ extern "C" int pnb_shade_tc_tables(void* ws, size_t ws_bytes, int max_valid_samp
     if (pack_cnt) *pack_cnt = w.pack_cnt;
     return PNB_OK;
 }
+// tests: device pointers of the pair kernel's products inside a workspace laid out for max_valid_samples (h-bar operand blocks, sigma)
+extern "C" int pnb_shade_tc_buffers(void* ws, size_t ws_bytes, int max_valid_samples, void** hbar, void** sigma) {
+    PNB_REQUIRE(ws && ws_bytes >= pnb_shade_tc_bytes(max_valid_samples), PNB_ERR_WORKSPACE, "pnb_shade_tc_buffers: workspace too small");
+    TcWs w(ws, ws_bytes, max_valid_samples);
+    if (hbar) *hbar = w.hbar;
+    if (sigma) *sigma = w.sigma;
+    return PNB_OK;
+}
 
 // Tensor-core forward: row packing, per-pair MLPs and colour branch on wgmma (BF16x3).  ws: >= pnb_shade_tc_bytes.
 extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pts, const pnb_mlp_t* mlp, const void* d_packed,

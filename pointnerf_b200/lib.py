@@ -68,7 +68,7 @@ FQ = dict(R2=0, n_bad_pixel=1)
 SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes", "pnb_grid_build", "pnb_query_bytes", "pnb_query",
            "pnb_query_export", "pnb_shade_bytes", "pnb_shade_forward", "pnb_composite_forward",
            "pnb_mlp_pack_bytes", "pnb_mlp_pack", "pnb_point_pre_bytes", "pnb_point_pre", "pnb_shade_tc_bytes", "pnb_shade_forward_tc",
-           "pnb_shade_tc_tables", "pnb_backward_bytes", "pnb_shade_backward", "pnb_backward_tables", "pnb_aux_outputs",
+           "pnb_shade_tc_tables", "pnb_shade_tc_buffers", "pnb_backward_bytes", "pnb_shade_backward", "pnb_backward_tables", "pnb_aux_outputs",
            "pnb_aux_conf_backward", "pnb_frustum_bytes", "pnb_frustum_build", "pnb_frustum_query_bytes", "pnb_frustum_query",
            "pnb_frustum_export"]
 # test-only library (csrc/selftest/pnb200_selftest.h)
@@ -144,6 +144,8 @@ def load():
     lib.pnb_shade_tc_tables.restype = C.c_int
     lib.pnb_shade_tc_tables.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                         C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.pnb_shade_tc_buffers.restype = C.c_int
+    lib.pnb_shade_tc_buffers.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     lib.pnb_backward_bytes.restype = C.c_size_t
     lib.pnb_backward_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.pnb_shade_backward.restype = C.c_int

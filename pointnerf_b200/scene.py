@@ -108,8 +108,19 @@ def make_intrinsic(cfg: SceneConfig):
     return np.array([[f, 0, cfg.W / 2], [0, f, cfg.H / 2], [0, 0, 1]], dtype=np.float32)
 
 
-def make_rays(cfg: SceneConfig, pixels=None):
+def orbit_rotation(yaw=0.7, pitch=0.3):
+    """camrotc2w [3,3] (fp32) of a camera orbited about the origin: yaw about the world y axis after pitch about x.  The shell configs'
+    cameras look at the origin along +z, so R @ cfg.campos looks at it along R[:, 2] and the shell stays between near and far."""
+    cy, sy, cp, sp = math.cos(yaw), math.sin(yaw), math.cos(pitch), math.sin(pitch)
+    Ry = np.array([[cy, 0.0, sy], [0.0, 1.0, 0.0], [-sy, 0.0, cy]])
+    Rx = np.array([[1.0, 0.0, 0.0], [0.0, cp, -sp], [0.0, sp, cp]])
+    return (Ry @ Rx).astype(np.float32)
+
+
+def make_rays(cfg: SceneConfig, pixels=None, camrotc2w=None):
     """pixels: None = full image in row-major (y outer, x inner) order, or an [R,2] array of (px,py).
+    camrotc2w: None (the identity camera of every config) or a [3,3] rotation (e.g. orbit_rotation()) that orbits the camera about the
+    origin: campos = R @ cfg.campos, raydir = R @ d_cam.
     Returns dict with raydir[1,R,3] f32 (un-normalised), pixel_idx[1,R,2] f32, campos[1,3],
     camrotc2w[1,3,3], intrinsic[1,3,3], near[1,1], far[1,1], h[1], w[1]."""
     K = make_intrinsic(cfg)
@@ -120,12 +131,14 @@ def make_rays(cfg: SceneConfig, pixels=None):
         pix = np.asarray(pixels, np.float32).reshape(-1, 2)
     x = (pix[:, 0] + 0.5 - K[0, 2]) / K[0, 0]
     y = (pix[:, 1] + 0.5 - K[1, 2]) / K[1, 1]
-    dirs = np.stack([x, y, np.ones_like(x)], axis=-1) @ np.eye(3, dtype=np.float32).T
+    rot = np.eye(3, dtype=np.float32) if camrotc2w is None else np.asarray(camrotc2w, np.float32).reshape(3, 3)
+    dirs = np.stack([x, y, np.ones_like(x)], axis=-1) @ rot.T
+    campos = cfg.campos if camrotc2w is None else tuple((rot @ np.asarray(cfg.campos, np.float32)).tolist())
     return dict(
         raydir=torch.from_numpy(dirs.astype(np.float32))[None],
         pixel_idx=torch.from_numpy(pix)[None],
-        campos=torch.tensor([cfg.campos], dtype=torch.float32),
-        camrotc2w=torch.eye(3)[None],
+        campos=torch.tensor([campos], dtype=torch.float32),
+        camrotc2w=torch.from_numpy(rot.copy())[None],
         intrinsic=torch.from_numpy(K)[None],
         near=torch.tensor([[cfg.near]], dtype=torch.float32),
         far=torch.tensor([[cfg.far]], dtype=torch.float32),

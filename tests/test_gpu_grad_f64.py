@@ -8,11 +8,10 @@ for outliers: a bug that touches a few pair rows only (a partial GEMM tile, one 
 F = 63 scatter) shows.  Each case reports how many units the kernel's masks flip against float64's own."""
 import ctypes as C
 
-import numpy as np
 import pytest
 import torch
 
-from oracle import grad_check, shade_oracle, shade_oracle_rw2c
+from oracle import forward_check, grad_check, shade_oracle, shade_oracle_rw2c
 from pointnerf_b200 import harness, lib, scene
 from pointnerf_b200.point_query import make_cam_opts
 
@@ -29,15 +28,7 @@ RTOL = {(0, "bf16x3"): (4e-5, 1.2e-4), (0, "fp32"): (4e-5, 1.2e-4), (4, "bf16x3"
         (1, "bf16x3"): (2e-5, 5e-6), (1, "fp32"): (2e-6, 3e-6)}
 
 
-def _dev_view(buf, ptr, dtype, shape):
-    """A CPU copy of a device array at address ptr inside the uint8 CUDA tensor buf."""
-    off = int(ptr) - buf.data_ptr()
-    n = int(np.prod(shape)) * torch.tensor([], dtype=dtype).element_size()
-    assert 0 <= off and off + n <= buf.numel()
-    return buf[off:off + n].view(dtype).view(*shape).cpu()
-
-
-def _kernel_masks(net, q, F):
+def _kernel_masks(net, q, F, camrotc2w):
     """The backward's masks as `slopes=` of the oracle (pair rows in the flattened [R',SR,K] order of sample_pidx >= 0, colour rows per
     sample slot), the dense export of the query, and the pair-row count."""
     l = lib.load()
@@ -45,29 +36,18 @@ def _kernel_masks(net, q, F):
     out = (C.c_void_p * 10)()
     ws = net._bwd_ws
     lib.check(l.pnb_backward_tables(ws.data_ptr(), ws.numel(), S, q.desc.cap_samples, F, out), "pnb_backward_tables")
-    H = [_dev_view(ws, out[0], torch.float32, (P, 256)), _dev_view(ws, out[1], torch.float32, (P, 272))[:, :256],
-         _dev_view(ws, out[2], torch.float32, (P, 256)), _dev_view(ws, out[3], torch.float32, (P, 256))]
-    Cc = [_dev_view(ws, out[i], torch.float32, (S, 128)) for i in (4, 5, 6)]
-    pair_off = _dev_view(ws, out[7], torch.int32, (S + 1,)).long()
-    row_samp = _dev_view(ws, out[8], torch.int32, (P,)).long()
-    pidx = _dev_view(ws, out[9], torch.int32, (P,)).long()
-    valid_list = _dev_view(q.ws, q.desc.valid_list, torch.int32, (S,)).long()
-    samp_off = _dev_view(q.ws, q.desc.samp_off, torch.int32, (q.R + 1,)).long()
-    ex = q.export(make_cam_opts(list(q.desc.campos), torch.eye(3)), want_pers=False, want_dirs=False)
-    ray_row = ex["ray_row"].cpu().long()
-    SR, K = q.SR, q.K
-    # valid sample -> (ray, sample slot) -> its row of the export
-    ray = torch.searchsorted(samp_off, valid_list, right=True) - 1
-    slot = valid_list - samp_off[ray]
-    srow = ray_row[ray] * SR + slot
-    # pair row -> (its sample, K slot)
-    assert pair_off[-1].item() == P
-    k = torch.arange(P) - pair_off[row_samp]
-    assert bool(((k >= 0) & (k < (pair_off[1:] - pair_off[:-1])[row_samp])).all())
-    flat = srow[row_samp] * K + k
-    pm = ex["sample_pidx"].cpu().reshape(-1).long()
-    assert torch.equal(torch.sort(flat)[0], (pm >= 0).nonzero()[:, 0]), "the packed rows are not the export's valid pairs"
-    assert torch.equal(pm[flat], pidx), "a packed row's point differs from the export's"
+    dev_view = forward_check.dev_view
+    H = [dev_view(ws, out[0], torch.float32, (P, 256)), dev_view(ws, out[1], torch.float32, (P, 272))[:, :256],
+         dev_view(ws, out[2], torch.float32, (P, 256)), dev_view(ws, out[3], torch.float32, (P, 256))]
+    Cc = [dev_view(ws, out[i], torch.float32, (S, 128)) for i in (4, 5, 6)]
+    pair_off = dev_view(ws, out[7], torch.int32, (S + 1,)).long()
+    row_samp = dev_view(ws, out[8], torch.int32, (P,)).long()
+    pidx = dev_view(ws, out[9], torch.int32, (P,)).long()
+    ex = q.export(make_cam_opts(list(q.desc.campos), camrotc2w), want_pers=False, want_dirs=False)
+    SR = q.SR
+    # valid sample -> (ray, sample slot) -> its row of the export; pair row -> (its sample, K slot)
+    srow = forward_check.sample_map(q, ex)["srow"]
+    flat = forward_check.pair_map(dict(srow=srow), pair_off, row_samp, pidx, ex, q.K)
     order = torch.argsort(flat)
     slopes = [torch.where(h[order] > 0, 1.0, 0.01).double() for h in H]
     for c in Cc:
@@ -92,7 +72,9 @@ def _loss(ray_color, conf_coefficient, opacity, bg_T, ext):
     return loss
 
 
-def _run_case(cfg_name, side, F=32, frames=False, order=2, mode=0, precision="bf16x3", ext=False, monkeypatch=None, **over):
+def _run_case(cfg_name, side, F=32, frames=False, order=2, mode=0, precision="bf16x3", ext=False, rotated=False, monkeypatch=None,
+              **over):
+    """rotated: the camera orbited about the origin (scene.orbit_rotation), so that camrotc2w is not the identity."""
     cfg = scene.CONFIGS[cfg_name]
     net, pts, opt = harness.build_model(cfg, DEV, alpha_bias=3.0, seed=2, feat_dim=F, agg_intrp_order=order, pnb_precision=precision,
                                         pnb_bwd_fp32=mode, **over)
@@ -101,20 +83,20 @@ def _run_case(cfg_name, side, F=32, frames=False, order=2, mode=0, precision="bf
     if frames:
         R = scene.edit_frames(pts["xyz"])
         npn.Rw2c = torch.nn.Parameter(R.to(DEV), requires_grad=False)
-    rays = scene.make_rays(cfg, scene.centre_patch(cfg, side))
+    rays = scene.make_rays(cfg, scene.centre_patch(cfg, side), camrotc2w=scene.orbit_rotation() if rotated else None)
+    cam = rays["camrotc2w"][0]
     out = _forward(net, rays)
     _loss(out["coarse_raycolor"][0], out["conf_coefficient"], out["coarse_point_opacity"][0], out["coarse_is_background"][0], ext).backward()
     net.check_errors()
     q = net.last
-    slopes, ex, P = _kernel_masks(net, q, F)
+    slopes, ex, P = _kernel_masks(net, q, F, cam)
     hit = ex["ray_mask"].cpu() > 0
     # float64 autograd through the oracle with the kernel's masks, on the kernel's own sample geometry
     pts_g = dict(xyz=npn.xyz.detach().cpu().double(), Rw2c=R.double())
     for k, t in (("embedding", npn.points_embeding), ("color", npn.points_color), ("dir", npn.points_dir), ("conf", npn.points_conf)):
         pts_g[k] = t.detach().cpu().double().requires_grad_(True)
     mlp_g = {k: v.double().requires_grad_(True) for k, v in harness.mlp_cpu(net.aggregator).items()}
-    args = (ex["sample_pidx"].cpu(), ex["sample_loc_w"].cpu(), rays["raydir"][0][hit], torch.tensor(cfg.campos), torch.eye(3), opt.vsize,
-            torch.ones(3))
+    args = (ex["sample_pidx"].cpu(), ex["sample_loc_w"].cpu(), rays["raydir"][0][hit], rays["campos"][0], cam, opt.vsize, torch.ones(3))
     sh = shade_oracle_rw2c.shade(pts_g, mlp_g, *args, dtype=torch.float64, agg_intrp_order=order, slopes=slopes)
     _loss(sh["ray_color"], sh["conf_coefficient"], sh["opacity"], sh["bg_T"], ext).backward()
     # float64's own masks: the units the kernel's masks flip (forward only)
@@ -138,10 +120,10 @@ def _run_case(cfg_name, side, F=32, frames=False, order=2, mode=0, precision="bf
         err[k] = grad_check.rel_error(p.grad.cpu(), mlp_g[k].grad)
     pts_worst = max(err[k] for k in ("embedding", "color", "dir", "conf"))
     mlp_worst = max(v for k, v in err.items() if "." in k)
-    max_nsamp = int(_dev_view(q.ws, q.desc.nsamp, torch.int32, (q.R,)).max())
-    print("\n[grad-f64] %s side=%d F=%d frames=%d order=%d mode=%d %s ext=%d %s: P=%d max nsamp=%d flips/layer=%s points=%.2e "
-          "mlp=%.2e (%s) conf0=%.2e/%.2e" % (cfg_name, side, F, frames, order, mode, precision, ext, over, P, max_nsamp, flips, pts_worst,
-                                             mlp_worst, max((k for k in err if "." in k), key=err.get), err0[0], err0[1]))
+    max_nsamp = int(forward_check.dev_view(q.ws, q.desc.nsamp, torch.int32, (q.R,)).max())
+    print("\n[grad-f64] %s side=%d F=%d frames=%d order=%d mode=%d %s ext=%d rot=%d %s: P=%d max nsamp=%d flips/layer=%s points=%.2e "
+          "mlp=%.2e (%s) conf0=%.2e/%.2e" % (cfg_name, side, F, frames, order, mode, precision, ext, rotated, over, P, max_nsamp, flips,
+                                             pts_worst, mlp_worst, max((k for k in err if "." in k), key=err.get), err0[0], err0[1]))
     rtol_points, rtol_mlp = RTOL[(mode, precision)]
     for k, v in err.items():
         rtol = rtol_mlp if "." in k else rtol_points
@@ -179,6 +161,15 @@ def test_chair_patch_beyond_four_split_k_slabs(F, mode, monkeypatch):
 @pytest.mark.parametrize("F", [32, 63])
 def test_edges(F, over, monkeypatch):
     _run_case("tiny", 16, F=F, monkeypatch=monkeypatch, **over)
+
+
+@pytest.mark.parametrize("mode", [0, 1])
+@pytest.mark.parametrize("frames", [False, True])
+@pytest.mark.parametrize("F", [32, 63])
+def test_backward_with_rotated_camera(F, frames, mode, monkeypatch):
+    """camrotc2w not the identity: the perspective coordinates, dists[3:6] and the ray-distance depth of every pair see the rotation
+    (rot3 and rot3T differ), and so do the opacity and bg_T terms of the loss."""
+    _run_case("tiny", 20, F=F, frames=frames, mode=mode, ext=True, rotated=True, monkeypatch=monkeypatch)
 
 
 @pytest.mark.parametrize("mode", [0, 1])
