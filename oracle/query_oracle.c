@@ -69,6 +69,7 @@ int pnb_oracle_query(
     const float* raypos,      /* optional R*D*3: if non-NULL these positions are used verbatim
                                  (the pybind op receives raypos, query_worldcoords.cpp:36) */
     int SR, int K,
+    int parity_slot0,         /* 1: slot 0 holds no points (.cu:147, Q1); 0: every stored voxel keeps its points */
     int8_t* ray_mask,         /* R */
     int* sample_pidx,         /* R*SR*K, first R2 rows valid, -1 padded */
     float* sample_loc_w,      /* R*SR*3, first R2 rows valid, zeros where unfilled */
@@ -126,7 +127,7 @@ int pnb_oracle_query(
                     coor_occ[(long)x * dim[1] * dim[2] + (long)y * dim[2] + z] = 1;
     }
 
-    /* ---- fill_occ2pnts (.cu:117-162), NOTE voxel_idx > 0 (.cu:147, Q1) ---- */
+    /* ---- fill_occ2pnts (.cu:117-162), NOTE voxel_idx > 0 (.cu:147, Q1) unless parity_slot0 is 0 ---- */
     int* raw_cnt = (int*)calloc((size_t)(n_slots > 0 ? n_slots : 1), sizeof(int));
     for (int i = 0; i < N; ++i) {
         int c0 = vox1(xyz[3 * i + 0], lo[0], svs[0]);
@@ -136,7 +137,7 @@ int pnb_oracle_query(
         long c = (long)c0 * dim[1] * dim[2] + (long)c1 * dim[2] + c2;
         int s = coor_2_occ[c];
         if (s >= 0) { raw_cnt[s]++; if (raw_cnt[s] > counters[1]) counters[1] = raw_cnt[s]; }
-        if (s > 0) {
+        if (s > 0 || (s == 0 && !parity_slot0)) {
             int tmp = occ_numpnts[s]++;
             if (tmp < P) occ_2_pnts[(long)s * P + tmp] = i;
             else counters[3] = 1;                   /* Q3: reference reservoir-samples; we keep first P */

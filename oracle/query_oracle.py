@@ -45,9 +45,11 @@ def _p(a, ty):
 
 
 def query(xyz, lo, svs, dim, kernel_size, query_size, max_o, P, radius_limit,
-          campos=None, raydir=None, t=None, raypos=None, SR=24, K=8):
+          campos=None, raydir=None, t=None, raypos=None, SR=24, K=8, parity_slot0=1):
     """Returns dict(sample_pidx[R2,SR,K] i32, sample_loc_w[R2,SR,3] f32, ray_mask[R] i8, counters{}).
-    t: [D] shared table or [R,D] per-ray table (train jitter).  raypos: optional [R,D,3]."""
+    t: [D] shared table or [R,D] per-ray table (train jitter).  raypos: optional [R,D,3].
+    parity_slot0: 1 = the voxel that wins occupancy slot 0 holds no points (query_worldcoords.cu:147, the reference's
+    behaviour); 0 = it keeps them (the product's pnb_parity_slot0 0)."""
     lib = _load()
     xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
     lo = np.ascontiguousarray(lo, np.float32); svs = np.ascontiguousarray(svs, np.float32)
@@ -79,7 +81,7 @@ def query(xyz, lo, svs, dim, kernel_size, query_size, max_o, P, radius_limit,
         _p(campos_a, ctypes.c_float), _p(raydir_a, ctypes.c_float), ctypes.c_int(R),
         _p(t_a, ctypes.c_float), ctypes.c_int(stride), ctypes.c_int(D),
         _p(raypos, ctypes.c_float),
-        ctypes.c_int(SR), ctypes.c_int(K),
+        ctypes.c_int(SR), ctypes.c_int(K), ctypes.c_int(1 if parity_slot0 else 0),
         _p(ray_mask, ctypes.c_int8), _p(pidx, ctypes.c_int), _p(loc, ctypes.c_float),
         _p(counters, ctypes.c_int))
     if rc != 0:

@@ -29,20 +29,41 @@ def run_oracle(name, pixels=None, **over):
     return cfg, s, opt, (ranges, svs, sdim, vscale, np.float32(rl ** 2), np.float32(dl ** 2)), out
 
 
-def brute_force(s, opt, grid, pixel_idx):
-    """Dilated occupancy as a set, candidates by explicit voxel membership, K nearest by float64 distance."""
+def fp32_distances(pts, loc):
+    """xy^2, z^2 and their sum in fp32 as the kernels form them (F9): fmaf(qx, qz, -cx*cz), fmaf(xv, xv, yv*yv), (qz - cz)^2.  Each fma
+    is evaluated in float64, where the product of two fp32 values and the sum with an fp32 value of similar size are exact, then
+    rounded once."""
+    f32, f64 = np.float32, np.float64
+    p = np.asarray(pts, f32).reshape(-1, 3).astype(f64)
+    cx, cy, cz = (f64(v) for v in np.asarray(loc, f32))
+    cxz, cyz = f64(f32(cx * cz)), f64(f32(cy * cz))
+    xv = (p[:, 0] * p[:, 2] - cxz).astype(f32).astype(f64)
+    yv = (p[:, 1] * p[:, 2] - cyz).astype(f32).astype(f64)
+    xy2 = (xv * xv + (yv * yv).astype(f32).astype(f64)).astype(f32)
+    dz = (p[:, 2] - cz).astype(f32)
+    z2 = (dz * dz).astype(f32)
+    return xy2, z2, (xy2 + z2).astype(f32)
+
+
+def brute_force(s, opt, grid, pixel_idx, pers=None):
+    """Dilated occupancy as a set, candidates by explicit voxel membership over the box the layered search covers for any accepted
+    kernel_size / query_size (x, y within (kernel_size[0] + 1) / 2 - 1 columns, z within (kernel_size[2] + 1) / 2 - 1 depths), K nearest
+    by float64 distance.  Each sample also carries its candidates as (fp32 distance of the kernels, index), sorted by that distance."""
     ranges, svs, sdim, vscale, r2, d2 = grid
     lo = ranges[:3]
-    q = (s["pers"] - lo) / svs                                    # float32, as the kernels form it
+    pers = s["pers"] if pers is None else pers
+    q = (pers - lo) / svs                                         # float32, as the kernels form it
     gx, gy, gz = (int(v) for v in sdim)
     fl = np.all((q >= 0) & (q < sdim), 1)
     tr = np.all((q > -1) & (q < sdim), 1)
     occ = {tuple(v) for v in np.floor(q[fl]).astype(int)}
+    qs, ks = opt.query_size, opt.kernel_size
+    hxy, hz = (ks[0] + 1) // 2 - 1, (ks[2] + 1) // 2 - 1
     cols = {}
     for (x, y, z) in occ:
-        for dx in range(-(opt.query_size[0] // 2), (opt.query_size[0] + 1) // 2):
-            for dy in range(-(opt.query_size[1] // 2), (opt.query_size[1] + 1) // 2):
-                for dz in range(-(opt.query_size[2] // 2), (opt.query_size[2] + 1) // 2):
+        for dx in range(-(qs[0] // 2), (qs[0] + 1) // 2):
+            for dy in range(-(qs[1] // 2), (qs[1] + 1) // 2):
+                for dz in range(-(qs[2] // 2), (qs[2] + 1) // 2):
                     X, Y, Z = x + dx, y + dy, z + dz
                     if 0 <= X < gx and 0 <= Y < gy and 0 <= Z < gz:
                         cols.setdefault((X, Y), set()).add(Z)
@@ -52,6 +73,9 @@ def brute_force(s, opt, grid, pixel_idx):
     rvs = (svs[:2].astype(np.float64) / vscale[:2]).astype(np.float32)
     mask, rows = [], []
     for px, py in pixel_idx:
+        if px < 0 or py < 0 or px // vscale[0] >= gx or py // vscale[1] >= gy:
+            mask.append(False)
+            continue
         c = cols.get((px // vscale[0], py // vscale[1]), set())
         m = bool(c) and max(c) > 0
         mask.append(m)
@@ -68,20 +92,23 @@ def brute_force(s, opt, grid, pixel_idx):
             loc = np.array([cx, cy, cz], np.float32)
             cand = []
             if fz >= 0:
-                for dx in (-1, 0, 1):
-                    for dy in (-1, 0, 1):
-                        for dz in (-1, 0, 1):
+                for dx in range(-hxy, hxy + 1):
+                    for dy in range(-hxy, hxy + 1):
+                        for dz in range(-hz, hz + 1):
                             v = (fx + dx, fy + dy, fz + dz)
                             if v in occ:
                                 cand += sorted(vox.get(v, []))[:opt.P]
-            pts = s["pers"][cand].astype(np.float64)
+            pts = pers[cand].astype(np.float64)
             L = loc.astype(np.float64)
             xy2 = (pts[:, 0] * pts[:, 2] - L[0] * L[2]) ** 2 + (pts[:, 1] * pts[:, 2] - L[1] * L[2]) ** 2
             z2 = (pts[:, 2] - L[2]) ** 2
             ok = ((r2 == 0) | (xy2 <= r2)) & ((d2 == 0) | (z2 <= d2))
+            xy32, z32, d32 = fp32_distances(pers[cand], loc)
+            ok32 = ((r2 == 0) | (xy32 <= r2)) & ((d2 == 0) | (z32 <= d2))
+            c32 = sorted(zip(d32[ok32].tolist(), np.asarray(cand, int)[ok32].tolist()), key=lambda e: e[0])
             cand, dist = np.asarray(cand, int)[ok], (xy2 + z2)[ok]
             order = np.argsort(dist, kind="stable")
-            ray.append((loc, cand[order], dist[order]))
+            ray.append((loc, cand[order], dist[order], c32))
         rows.append(ray)
     return np.asarray(mask, np.int8), rows
 
@@ -96,7 +123,7 @@ def test_oracle_matches_brute_force(name):
     assert out["counters"]["overflow_p"] == 0 and out["counters"]["overflow_o"] == 0
     near_ties = 0
     for r, ray in enumerate(rows):
-        for j, (loc, cand, dist) in enumerate(ray):
+        for j, (loc, cand, dist, _) in enumerate(ray):
             np.testing.assert_array_equal(out["sample_loc"][r, j], loc)
             got = set(int(v) for v in out["sample_pidx"][r, j] if v >= 0)
             want = set(int(v) for v in cand[:opt.K])

@@ -1,6 +1,7 @@
 """CPU: pins oracle/query_oracle.c (serial C restatement of query_worldcoords.cu) against an independent
 brute-force numpy formulation of the canonical semantics (SURVEY.md 8a) and against the committed fixtures
-that were produced through the reference's own lighting_fast_querier class (oracle/make_golden.py)."""
+that were produced through the reference's own lighting_fast_querier class (oracle/make_golden.py).
+The brute force does not restate the tie rule: tests/test_query_ties_oracle.py pins it with hand-built cases."""
 import os
 
 import numpy as np
@@ -12,8 +13,11 @@ from pointnerf_b200 import scene
 from oracle import golden  # noqa: E402
 
 
-def brute_force(xyz, lo, svs, dim, ks, qs, P, r, campos, raydir, t, SR, K):
-    """Independent formulation: dict-of-lists voxel map, numpy distance sort (stable), shell by shell."""
+def brute_force(xyz, lo, svs, dim, ks, qs, P, r, campos, raydir, t, SR, K, parity_slot0=1):
+    """Independent formulation: dict-of-lists voxel map, shell by shell, fp32 distances formed as the SASS forms them.
+    Returns the ray mask [R], the sample positions [R2,SR,3] and, per kept ray and sample, every candidate (d2, index) of the visited
+    shells sorted by distance (stable in visit order): which K of them the kernel keeps where the K-th distance ties is decided by its
+    replace-farthest rule, and check_sets() pins only what does not depend on that rule."""
     f32 = np.float32
     vox = np.floor(((xyz - lo.astype(f32)).astype(f32) / svs.astype(f32)).astype(f32)).astype(np.int64)
     inside = np.all((vox >= 0) & (vox < dim), axis=1)
@@ -29,24 +33,26 @@ def brute_force(xyz, lo, svs, dim, ks, qs, P, r, campos, raydir, t, SR, K):
             for b in range(max(0, y - qs[1] // 2), min(dim[1], y + (qs[1] + 1) // 2)):
                 for c in range(max(0, z - qs[2] // 2), min(dim[2], z + (qs[2] + 1) // 2)):
                     occ.add((a, b, c))
-    stored = {k: v[:P] for k, v in cells.items() if k != first_cell}   # Q1: slot 0 holds nothing
+    # Q1: the voxel of the lowest in-range index wins occupancy slot 0 and holds nothing (unless parity_slot0 is off)
+    stored = {k: v[:P] for k, v in cells.items() if k != first_cell or not parity_slot0}
     r2 = f32(r) * f32(r)
     res_mask = np.zeros(len(raydir), np.int8)
-    res_pidx, res_loc = [], []
+    res_loc, res_found = [], []
+    t = np.asarray(t, f32)
     for ri in range(len(raydir)):
-        pos = (campos.astype(f32)[None] + (raydir[ri].astype(f32)[None] * t.astype(f32)[:, None]).astype(f32)).astype(f32)
+        tr = t[ri] if t.ndim == 2 else t
+        pos = (campos.astype(f32)[None] + (raydir[ri].astype(f32)[None] * tr[:, None]).astype(f32)).astype(f32)
         v = np.floor(((pos - lo.astype(f32)).astype(f32) / svs.astype(f32)).astype(f32)).astype(np.int64)
-        hits = [d for d in range(len(t)) if np.all(v[d] >= 0) and np.all(v[d] < dim) and tuple(v[d]) in occ]
+        hits = [d for d in range(len(tr)) if np.all(v[d] >= 0) and np.all(v[d] < dim) and tuple(v[d]) in occ]
         if not hits:
             continue
         hits = hits[:SR]
-        pidx = -np.ones((SR, K), np.int32)
         loc = np.zeros((SR, 3), f32)
+        ray = []
         for s, d in enumerate(hits):
             loc[s] = pos[d]
             f = v[d]
-            found = []  # (d2, traversal order, idx)
-            order = 0
+            found = []  # (d2, idx) in visit order
             for layer in range((ks[0] + 1) // 2):
                 for x in range(max(-f[0], -layer), min(dim[0] - f[0], layer + 1)):
                     for y in range(max(-f[1], -layer), min(dim[1] - f[1], layer + 1)):
@@ -59,19 +65,37 @@ def brute_force(xyz, lo, svs, dim, ks, qs, P, r, campos, raydir, t, SR, K):
                                 d2 = f32(np.float64(dv[2]) * np.float64(dv[2]) + np.float64(
                                     f32(np.float64(dv[0]) * np.float64(dv[0]) + np.float64(yy))))
                                 if r2 == 0 or d2 <= r2:
-                                    found.append((d2, order, i))
-                                    order += 1
+                                    found.append((float(d2), int(i)))
                 if len(found) >= K:
                     break
-            # replace-farthest with strict '<' keeps the K smallest, earliest wins ties
-            found.sort(key=lambda e: (e[0], e[1]))
-            keep = found[:K]
-            pidx[s, :len(keep)] = sorted(e[2] for e in keep)
-        if np.any(pidx >= 0):
+            ray.append(sorted(found, key=lambda e: e[0]))
+        if any(ray):
             res_mask[ri] = 1
-            res_pidx.append(pidx)
             res_loc.append(loc)
-    return res_mask, np.array(res_pidx), np.array(res_loc)
+            res_found.append(ray)
+    return res_mask, np.array(res_loc, f32).reshape(-1, SR, 3), res_found
+
+
+def check_sets(pidx, found, K):
+    """The oracle's neighbour sets [R2,SR,K] against brute_force's candidates.  Where the K-th smallest distance is not tied the K
+    nearest are one set and must match exactly.  Where it ties, every candidate nearer than the tied distance must be kept and the
+    rest of the K must sit at the tied distance; which of the tied ones stay is the replace-farthest rule's choice, pinned by the
+    hand-built cases of test_query_ties_oracle.py.  Returns the number of tied samples."""
+    tied = 0
+    for r, ray in enumerate(found):
+        for s in range(pidx.shape[1]):
+            cand = ray[s] if s < len(ray) else []
+            got = sorted(int(v) for v in pidx[r, s] if v >= 0)
+            if len(cand) <= K or cand[K - 1][0] != cand[K][0]:
+                assert got == sorted(i for _, i in cand[:K]), (r, s, got, cand[:K + 1])
+                continue
+            tied += 1
+            dk = cand[K - 1][0]
+            below = {i for d, i in cand if d < dk}
+            at = {i for d, i in cand if d == dk}
+            g = set(got)
+            assert len(got) == K and below <= g and (g - below) <= at, (r, s, got, cand[:K + 1])
+    return tied
 
 
 def _setup(cfg, pixels, SR=24, K=8, P=None):
@@ -92,11 +116,11 @@ def test_oracle_vs_bruteforce(K, SR, P):
     r = float(pipeline.radius_limit(4.0, [cfg.vsize] * 3))
     o = query_oracle.query(pts["xyz"].numpy(), rng6[:3], svs, dim, ks, qs, 100000, P, r, campos=np.array(cfg.campos),
                            raydir=rays["raydir"][0].numpy(), t=t, SR=SR, K=K)
-    m, pidx, loc = brute_force(pts["xyz"].numpy(), rng6[:3], svs, dim, ks, qs, P, r, np.array(cfg.campos, np.float32),
-                               rays["raydir"][0].numpy(), t, SR, K)
+    m, loc, found = brute_force(pts["xyz"].numpy(), rng6[:3], svs, dim, ks, qs, P, r, np.array(cfg.campos, np.float32),
+                                rays["raydir"][0].numpy(), t, SR, K)
     assert np.array_equal(m, o["ray_mask"])
-    assert o["sample_pidx"].shape == pidx.shape
-    assert np.array_equal(np.sort(o["sample_pidx"], axis=-1), np.sort(pidx, axis=-1))
+    assert o["sample_pidx"].shape[0] == loc.shape[0]
+    assert check_sets(o["sample_pidx"], found, K) == 0           # a smooth random cloud: no distance ties at all
     assert np.array_equal(o["sample_loc_w"], loc)
     if P == 2:
         assert o["counters"]["overflow_p"] == 1
