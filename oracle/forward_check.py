@@ -9,6 +9,8 @@ instead:
   decode_hbar            h-bar as the pair kernel hands it to the colour kernel (bf16 hi + lo operand blocks);
   march                  the ray-distance + ray_march tail of shade_oracle.shade on a given (sigma, rgb), so that the compositing kernel
                          is checked on the shading kernel's own output;
+  edit_*                 point values a trained checkpoint has and the generator does not (conf outside its clamp, embeddings of several
+                         units, non-unit and zero directions, colours outside [0, 1]), written into a built model in place;
   sample_errors / check  errors per valid sample relative to the case's scale, with no outlier allowance; a failure names the worst
                          sample's ray, slot, valid index, colour tile and row, and neighbour count.
 The forward needs no LeakyReLU masks (unlike the backward, oracle/grad_check.py): LeakyReLU is 1-Lipschitz, so a unit that rounding
@@ -88,10 +90,10 @@ def decode_hbar(ws, n_valid):
     return torch.from_numpy(_bf16(b, off).astype(np.float64) + _bf16(b, off + 8192).astype(np.float64))
 
 
-def march(decoded, ray_valid, sample_loc_w, campos, camrotc2w, vsize, bg_color, dtype=torch.float64):
+def march(decoded, ray_valid, sample_loc_w, campos, camrotc2w, vsize, bg_color, dtype=torch.float64, raydist_mode_unit=1):
     """The ray-distance and ray_march tail of shade_oracle.shade on a given decoded [R',SR,4] (sigma, rgb).  The one discontinuous
-    choice, the raydist_mode_unit mask (< 1e-8 or > 2 vz), is taken on fp32 distances as the reference takes it; the rest runs in
-    `dtype`.  In fp32 this is shade()'s own arithmetic."""
+    choice, the ray-distance mask (< 1e-8 or, with raydist_mode_unit, > 2 vz), is taken on fp32 distances as the reference takes it; the
+    rest runs in `dtype`.  In fp32 this is shade()'s own arithmetic."""
     vz = float(vsize[2])
     Rn = decoded.shape[0]
     cam = camrotc2w.reshape(3, 3)
@@ -102,7 +104,10 @@ def march(decoded, ray_valid, sample_loc_w, campos, camrotc2w, vsize, bg_color, 
         return torch.cat([z[..., 1:] - z[..., :-1], torch.full((Rn, 1), vz, dtype=dt)], dim=-1)
 
     d32 = steps(torch.float32)
-    m = torch.logical_or(d32 < 1e-8, d32 > 2 * vz).to(dtype)
+    m = d32 < 1e-8
+    if raydist_mode_unit > 0:
+        m = torch.logical_or(m, d32 > 2 * vz)
+    m = m.to(dtype)
     ray_dist = d32.to(dtype) if dtype == torch.float32 else steps(dtype)
     ray_dist = ray_dist * (1.0 - m) + m * vz
     ray_dist = ray_dist * ray_valid.to(dtype)
@@ -115,6 +120,42 @@ def march(decoded, ray_valid, sample_loc_w, campos, camrotc2w, vsize, bg_color, 
     blend_weight = (opacity * acc_T)[..., None]
     ray_color = torch.sum(decoded[..., 1:4] * blend_weight, dim=-2) + bg_color.to(dtype).view(1, 3) * bg_T
     return dict(ray_dist=ray_dist, opacity=opacity, bg_T=bg_T, blend_weight=blend_weight, ray_color=ray_color)
+
+
+def edit_conf(net, rays=None):
+    """5 % of points_conf outside the clamp (0.0001, 1): zero, negative, tiny positive, above 1."""
+    c = net.neural_points.points_conf
+    N = c.shape[1]
+    g = torch.Generator().manual_seed(7)
+    idx = torch.randperm(N, generator=g)[:N // 20]
+    vals = torch.tensor([0.0, -0.3, 5e-5, 1.7, 1.0 + 1e-3, -1e-6, 9.99e-5, 30.0])
+    with torch.no_grad():
+        c[0, idx.to(c.device), 0] = vals.repeat(len(idx) // len(vals) + 1)[:len(idx)].to(c.device)
+
+
+def edit_embedding(scale):
+    """points_embeding times `scale` (the generator's is 0.5 randn; the PE of the features takes 4 f)."""
+    def edit(net, rays=None):
+        with torch.no_grad():
+            net.neural_points.points_embeding.mul_(scale)
+    return edit
+
+
+def edit_dir(net, rays=None):
+    """points_dir of every point scaled by a seeded factor in [0, 3], 2 % of the points exactly zero."""
+    d = net.neural_points.points_dir
+    N = d.shape[1]
+    g = torch.Generator().manual_seed(8)
+    f = 3.0 * torch.rand(N, generator=g)
+    f[torch.randperm(N, generator=g)[:N // 50]] = 0.0
+    with torch.no_grad():
+        d.mul_(f.to(d.device)[None, :, None])
+
+
+def edit_color(net, rays=None):
+    """points_color from [0, 1] to [-0.5, 1.5]."""
+    with torch.no_grad():
+        net.neural_points.points_color.mul_(2.0).sub_(0.5)
 
 
 def sample_errors(got, ref, rows):

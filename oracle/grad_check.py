@@ -35,10 +35,11 @@ def check_points(a, ref, name, rtol):
     return float(e.max())
 
 
-def point0_conf_bound(n0, ref0):
+def point0_conf_bound(n0, ref0, term=1e-3):
     """Bound of the error of an fp32 sum into point 0's conf gradient: n0 terms (one per gathered slot), each rounding step off by at
-    most U32 of the partial sum, which stays below |ref0| plus the padded terms' 1e-3 each (the loss's 1e-3 * conf_coefficient.sum())."""
-    return n0 * U32 * (abs(float(ref0)) + 1e-3 * n0)
+    most U32 of the partial sum, which stays below |ref0| plus the padded terms' `term` each (1e-3: the loss's
+    1e-3 * conf_coefficient.sum())."""
+    return n0 * U32 * (abs(float(ref0)) + term * n0)
 
 
 def check_conf(a, ref, n0, rtol):

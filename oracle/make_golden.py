@@ -48,9 +48,9 @@ def build_reference_net(cfg, alpha_bias, SR=24, is_train=False, extra_flags=()):
     return net, agg, npts, pts, opt
 
 
-def golden_case(name, cfg, pixels, alpha_bias, SR=24, extra_flags=()):
+def golden_case(name, cfg, pixels, alpha_bias, SR=24, extra_flags=(), bg_color=(1.0, 1.0, 1.0)):
     net, agg, npts, pts, opt = build_reference_net(cfg, alpha_bias, SR=SR, extra_flags=extra_flags)
-    rays = scene.make_rays(cfg, pixels)
+    rays = scene.make_rays(cfg, pixels, bg_color=bg_color)
     out = net(rays["campos"], rays["raydir"], bg_color=rays["bg_color"], camrotc2w=rays["camrotc2w"],
               pixel_idx=rays["pixel_idx"], near=rays["near"], far=rays["far"], h=rays["h"], w=rays["w"],
               intrinsic=rays["intrinsic"])
@@ -65,6 +65,7 @@ def golden_case(name, cfg, pixels, alpha_bias, SR=24, extra_flags=()):
     g = {n: p.grad for n, p in net.named_parameters() if p.grad is not None}
     fx = dict(
         alpha_bias=np.float32(alpha_bias), SR=np.int32(SR), pixels=np.asarray(pixels, np.float32), agg_intrp_order=np.int32(opt.agg_intrp_order),
+        raydist_mode_unit=np.int32(opt.raydist_mode_unit), bg_color=np.asarray(bg_color, np.float32),
         ranges6=rng_t.detach().numpy(), scaled_vdim=sdim, counters=np.array([query_oracle.last_counters[k] for k in query_oracle.COUNTER_NAMES], np.int32),
         ray_mask=out["ray_mask"][0].numpy(), sample_pidx=qp[0][0].numpy(), sample_loc=qp[1][0].detach().numpy(),
         sample_loc_w=qp[2][0].numpy(),
@@ -169,11 +170,19 @@ if __name__ == "__main__":
         tiny = scene.CONFIGS["tiny"]
         golden_case("tiny_order1", tiny, scene.centre_patch(tiny, 40), alpha_bias=4.0, extra_flags=["--agg_intrp_order", "1"])
         sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "raydist0_bg":
+        tiny = scene.CONFIGS["tiny"]
+        golden_case("tiny_raydist0_bg", tiny, scene.centre_patch(tiny, 40), alpha_bias=4.0, extra_flags=["--raydist_mode_unit", "0"],
+                    bg_color=(0.9, 0.1, 0.4))
+        sys.exit(0)
     tiny = scene.CONFIGS["tiny"]
     golden_case("tiny_opaque", tiny, scene.centre_patch(tiny, 40), alpha_bias=4.0)
     golden_case("tiny_thin_sr8", tiny, scene.centre_patch(tiny, 40), alpha_bias=0.0, SR=8)
     # agg_intrp_order = 1 (point_aggregators.py:573-599: alpha_branch on the K-aggregated feature), SURVEY 8(f) rank 4
     golden_case("tiny_order1", tiny, scene.centre_patch(tiny, 40), alpha_bias=4.0, extra_flags=["--agg_intrp_order", "1"])
+    # the reference's default ray distances (raydist_mode_unit 0: a step above 2 vsize_z stays) and a background of three different channels
+    golden_case("tiny_raydist0_bg", tiny, scene.centre_patch(tiny, 40), alpha_bias=4.0, extra_flags=["--raydist_mode_unit", "0"],
+                bg_color=(0.9, 0.1, 0.4))
     golden_probe("tiny_probe", tiny, scene.centre_patch(tiny, 40), alpha_bias=4.0)
     golden_hyper()
     golden_checkpoint_layout()

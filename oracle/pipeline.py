@@ -44,7 +44,7 @@ def radius_limit(radius_limit_scale, vsize):
 
 def render(points, mlp, raydir, campos, camrotc2w, near, far, vsize, vscale, kernel_size, query_size,
            ranges, SR, K, P, max_o, D=400, radius_limit_scale=4.0, bg_color=(1., 1., 1.), t=None,
-           dtype=torch.float32, want_shade=True, agg_intrp_order=2):
+           dtype=torch.float32, want_shade=True, agg_intrp_order=2, raydist_mode_unit=1):
     """raydir [R,3] torch f32.  Returns dict: query outputs + shade outputs + fill_invalid outputs + counters."""
     rng6, svs, dim = hyperparameters(points["xyz"], vsize, vscale, kernel_size, ranges)
     if t is None:
@@ -69,7 +69,7 @@ def render(points, mlp, raydir, campos, camrotc2w, near, far, vsize, vscale, ker
         return out
     sh = shade_oracle.shade(points, mlp, torch.from_numpy(q["sample_pidx"]), torch.from_numpy(q["sample_loc_w"]),
                             raydir[mask], torch.as_tensor(campos), torch.as_tensor(camrotc2w), vsize,
-                            torch.as_tensor(bg_color), dtype=dtype, agg_intrp_order=agg_intrp_order)
+                            torch.as_tensor(bg_color), dtype=dtype, agg_intrp_order=agg_intrp_order, raydist_mode_unit=raydist_mode_unit)
     out.update(sh)
     out.update(shade_oracle.fill_invalid(mask, sh["ray_color"], sh["opacity"], sh["bg_T"], sh["queried_shading"],
                                          torch.as_tensor(bg_color)))

@@ -17,11 +17,11 @@ from . import shade_oracle
 
 
 def shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w, vsize, bg_color,
-          dtype=torch.float32, agg_intrp_order=2, slopes=None):
+          dtype=torch.float32, agg_intrp_order=2, slopes=None, raydist_mode_unit=1):
     """The arguments and the returned dict of shade_oracle.shade; points["Rw2c"] is [3,3] or [N,3,3]."""
     if points["Rw2c"].dim() == 2:
         return shade_oracle.shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w, vsize, bg_color,
-                                  dtype=dtype, agg_intrp_order=agg_intrp_order, slopes=slopes)
+                                  dtype=dtype, agg_intrp_order=agg_intrp_order, slopes=slopes, raydist_mode_unit=raydist_mode_unit)
     assert agg_intrp_order in (1, 2)
     cv = lambda t: t.to(dtype)
     xyz = cv(points["xyz"]); emb = cv(points["embedding"][0]); col = cv(points["color"][0])
@@ -104,7 +104,10 @@ def shade(points, mlp, sample_pidx, sample_loc_w, raydir_hit, campos, camrotc2w,
     vz = float(vsize[2])
     z = torch.cummax(sample_loc[..., 2], dim=-1)[0]
     ray_dist = torch.cat([z[..., 1:] - z[..., :-1], torch.full((Rn, 1), vz, dtype=dtype)], dim=-1)
-    m = torch.logical_or(ray_dist < 1e-8, ray_dist > 2 * vz).to(dtype)
+    m = ray_dist < 1e-8
+    if raydist_mode_unit > 0:
+        m = torch.logical_or(m, ray_dist > 2 * vz)
+    m = m.to(dtype)
     ray_dist = ray_dist * (1.0 - m) + m * vz
     ray_dist = ray_dist * ray_valid.to(dtype)
 

@@ -117,12 +117,12 @@ def orbit_rotation(yaw=0.7, pitch=0.3):
     return (Ry @ Rx).astype(np.float32)
 
 
-def make_rays(cfg: SceneConfig, pixels=None, camrotc2w=None):
+def make_rays(cfg: SceneConfig, pixels=None, camrotc2w=None, bg_color=(1.0, 1.0, 1.0)):
     """pixels: None = full image in row-major (y outer, x inner) order, or an [R,2] array of (px,py).
     camrotc2w: None (the identity camera of every config) or a [3,3] rotation (e.g. orbit_rotation()) that orbits the camera about the
-    origin: campos = R @ cfg.campos, raydir = R @ d_cam.
+    origin: campos = R @ cfg.campos, raydir = R @ d_cam.  bg_color: the three channels of the background (white by default).
     Returns dict with raydir[1,R,3] f32 (un-normalised), pixel_idx[1,R,2] f32, campos[1,3],
-    camrotc2w[1,3,3], intrinsic[1,3,3], near[1,1], far[1,1], h[1], w[1]."""
+    camrotc2w[1,3,3], intrinsic[1,3,3], near[1,1], far[1,1], h[1], w[1], bg_color[1,3]."""
     K = make_intrinsic(cfg)
     if pixels is None:
         px, py = np.meshgrid(np.arange(cfg.W).astype(np.float32), np.arange(cfg.H).astype(np.float32))
@@ -143,7 +143,7 @@ def make_rays(cfg: SceneConfig, pixels=None, camrotc2w=None):
         near=torch.tensor([[cfg.near]], dtype=torch.float32),
         far=torch.tensor([[cfg.far]], dtype=torch.float32),
         h=torch.tensor([cfg.H]), w=torch.tensor([cfg.W]),
-        bg_color=torch.ones(1, 3),
+        bg_color=torch.tensor([list(bg_color)], dtype=torch.float32),
     )
 
 

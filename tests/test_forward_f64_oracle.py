@@ -2,8 +2,9 @@
 
 The fp32 oracle agrees with float64 on every sample without any LeakyReLU masks; forward_check.march reproduces shade()'s compositing bit
 for bit; defects that the 1e-4 rule on radiance and opacity lets through (one K slot dropped, every sigma 3e-4 too large, one h-bar
-channel of one sample off by 1e-3 of scale) fail the per-sample check; decode_hbar reads the colour kernel's operand layout; and the
-orbited camera of the GPU tests hits the shell and changes the oracle's outputs."""
+channel of one sample off by 1e-3 of scale) fail the per-sample check; decode_hbar reads the colour kernel's operand layout; the
+orbited camera of the GPU tests hits the shell and changes the oracle's outputs; and defects in the use of bg_color that no comparison
+sees under a white background fail the per-ray comparison under (0.9, 0.1, 0.4)."""
 import numpy as np
 import pytest
 import torch
@@ -18,9 +19,9 @@ RTOL_FP32 = dict(sigma=1.5e-6, rgb=6e-7, hbar=4e-6)
 OLD_TOL = 1e-4
 
 
-def _case(F=32, order=2, frames=False, rotated=True, alpha_bias=3.0, side=20):
+def _case(F=32, order=2, frames=False, rotated=True, alpha_bias=3.0, side=20, pixels=None, **over):
     cfg = scene.CONFIGS["tiny"]
-    opt = harness.make_opt(cfg, feat_dim=F, agg_intrp_order=order)
+    opt = harness.make_opt(cfg, feat_dim=F, agg_intrp_order=order, **over)
     agg = PointAggregator(opt, seed=2)
     with torch.no_grad():
         agg.alpha_branch[0].bias += alpha_bias
@@ -32,7 +33,8 @@ def _case(F=32, order=2, frames=False, rotated=True, alpha_bias=3.0, side=20):
         pts["embedding"] = torch.cat([pts["color"], pts["dir"], pts["conf"], pts["embedding"]], dim=-1)
     if frames:
         pts["Rw2c"] = scene.edit_frames(pts["xyz"])
-    rays = scene.make_rays(cfg, scene.centre_patch(cfg, side), camrotc2w=scene.orbit_rotation() if rotated else None)
+    rays = scene.make_rays(cfg, scene.centre_patch(cfg, side) if pixels is None else pixels,
+                           camrotc2w=scene.orbit_rotation() if rotated else None)
     cam, campos = rays["camrotc2w"][0], rays["campos"][0]
     q = pipeline.render(pts, mlp, rays["raydir"][0], campos.numpy(), cam.numpy(), cfg.near, cfg.far, opt.vsize, opt.vscale,
                         opt.kernel_size, opt.query_size, opt.ranges, opt.SR, opt.K, opt.P, cfg.N, D=cfg.D, want_shade=False)
@@ -41,7 +43,7 @@ def _case(F=32, order=2, frames=False, rotated=True, alpha_bias=3.0, side=20):
             torch.ones(3))
     shade = shade_oracle_rw2c.shade if frames else shade_oracle.shade
     run = lambda dtype, a=args: shade(pts, mlp, *a, dtype=dtype, agg_intrp_order=order)
-    return dict(run=run, args=args, pts=pts, mlp=mlp, order=order, sh32=run(torch.float32), sh64=run(torch.float64))
+    return dict(run=run, args=args, pts=pts, mlp=mlp, order=order, mask=mask, sh32=run(torch.float32), sh64=run(torch.float64))
 
 
 def _rows(sh):
@@ -53,8 +55,9 @@ def _got(sh, rows, decoded=None, hbar=None):
     return dict(sigma=dec[:, 0], rgb=dec[:, 1:], hbar=(sh["hbar"] if hbar is None else hbar)[rows])
 
 
-def _march(c, decoded, dtype=torch.float32):
-    _, loc_w, _, campos, cam, vsize, bg = c["args"]
+def _march(c, decoded, dtype=torch.float32, bg=None):
+    _, loc_w, _, campos, cam, vsize, bg0 = c["args"]
+    bg = bg0 if bg is None else bg
     return forward_check.march(decoded, c["sh32"]["ray_valid"], loc_w, campos, cam, vsize, bg, dtype=dtype)
 
 
@@ -191,3 +194,47 @@ def test_rotated_camera_matters():
     d = max((ident[k] - c["sh32"][k]).abs().max().item() for k in ("ray_color", "opacity", "bg_T"))
     assert d > 100 * OLD_TOL, d
     assert float(c["sh32"]["bg_T"].min()) < 0.9
+
+
+@pytest.mark.parametrize("defect", ["channels_0_2_swapped", "white_on_missed_rays"])
+def test_background_defects_need_a_coloured_background(defect):
+    """bg_color with its channels 0 and 2 swapped in the compositing, and missed rays painted 1 instead of bg_color: under the white
+    background every ray agrees bit for bit, under (0.9, 0.1, 0.4) the per-ray comparison fails."""
+    cfg = scene.CONFIGS["tiny"]
+    side = 20
+    c = _case(pixels=scene.centre_patch(cfg, side) + np.float32([side // 2, 0]))       # across the limb of the shell
+    mask = c["mask"]
+    assert 0 < int(mask.sum()) < mask.numel(), "the patch needs hit and missed rays"
+    dec = c["sh32"]["decoded"]
+
+    def full(bg_march, bg_fill):
+        m = _march(c, dec, bg=bg_march)
+        return shade_oracle.fill_invalid(mask, m["ray_color"], m["opacity"], m["bg_T"], torch.zeros(int(mask.sum()), 3), bg_fill)["coarse_raycolor"]
+
+    for bg in (torch.ones(3), torch.tensor([0.9, 0.1, 0.4])):
+        ref = full(bg, bg)
+        bad = full(bg.flip(0), bg) if defect == "channels_0_2_swapped" else full(bg, torch.ones(3))
+        errs = dict(composite=(bad - ref).abs().amax(-1))
+        if bool((bg == 1).all()):
+            assert torch.equal(bad, ref)
+        else:
+            with pytest.raises(AssertionError, match="composite"):
+                forward_check.check(errs, dict(composite=1e-5))
+
+
+def test_raydist_mode_unit_0_keeps_the_long_steps():
+    """raydist_mode_unit 0 drops the `> 2 vsize_z` replacement only: the shell's front-to-back step stays (tens of voxels), every other
+    step is the unit mode's, march follows shade, and the default is the unit mode.  SR 80: 24 slots end inside the front crossing."""
+    c = _case(side=12, SR=80)
+    pidx, loc_w, raydir, campos, cam, vsize, bg = c["args"]
+    sh0 = shade_oracle.shade(c["pts"], c["mlp"], *c["args"], raydist_mode_unit=0)
+    sh1 = c["sh32"]
+    assert torch.equal(shade_oracle.shade(c["pts"], c["mlp"], *c["args"], raydist_mode_unit=1)["ray_color"], sh1["ray_color"])
+    vz = float(vsize[2])
+    long = sh0["ray_dist"] > 2 * vz
+    assert int(long.sum()) > 50 and float(sh0["ray_dist"].max()) > 10 * vz
+    assert torch.equal(sh0["ray_dist"][~long], sh1["ray_dist"][~long]) and bool((sh1["ray_dist"][long] == vz).all())
+    assert (sh0["ray_color"] - sh1["ray_color"]).abs().max().item() > 100 * OLD_TOL
+    m = forward_check.march(sh0["decoded"], sh0["ray_valid"], loc_w, campos, cam, vsize, bg, dtype=torch.float32, raydist_mode_unit=0)
+    for k in ("ray_dist", "opacity", "bg_T", "blend_weight", "ray_color"):
+        assert torch.equal(m[k], sh0[k]), k

@@ -41,7 +41,7 @@ def _forward(net, cfg, rays):
 
 
 @pytest.mark.parametrize("precision,bwd_fp32", [("bf16x3", 0), ("bf16x3", 1), ("bf16x3", 4), ("fp32", 0)])
-@pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1"])
+@pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1", "tiny_raydist0_bg"])
 def test_gradients_match_reference_fixture(name, precision, bwd_fp32, golden_dir):
     """bwd_fp32 = 0: every layer GEMM of the backward on the tensor cores (wgmma, BF16x3; default); 4: the forward recompute on the
     fp32 CUDA-core tiles (fp32-faithful LeakyReLU masks), dX / dW on the tensor cores; 1: everything on the fp32 tiles.  Modes 1 and 4
@@ -49,9 +49,13 @@ def test_gradients_match_reference_fixture(name, precision, bwd_fp32, golden_dir
     fx = golden.load(golden_dir, name)
     cfg = scene.CONFIGS["tiny"]
     order = int(fx["agg_intrp_order"]) if "agg_intrp_order" in fx.files else 2       # tiny_order1: the reference run with --agg_intrp_order 1
-    net, pts, opt = harness.build_model(cfg, DEV, SR=int(fx["SR"]), max_o=100000, pnb_precision=precision, pnb_bwd_fp32=bwd_fp32, agg_intrp_order=order)
+    # tiny_raydist0_bg: the reference run with --raydist_mode_unit 0 and bg_color (0.9, 0.1, 0.4)
+    mode_unit = int(fx["raydist_mode_unit"]) if "raydist_mode_unit" in fx.files else 1
+    bg = fx["bg_color"].tolist() if "bg_color" in fx.files else (1.0, 1.0, 1.0)
+    net, pts, opt = harness.build_model(cfg, DEV, SR=int(fx["SR"]), max_o=100000, pnb_precision=precision, pnb_bwd_fp32=bwd_fp32, agg_intrp_order=order,
+                                        raydist_mode_unit=mode_unit)
     net.aggregator.load_state_dict({k[4:]: torch.from_numpy(fx[k]) for k in fx.files if k.startswith("mlp.")})
-    out = _forward(net, cfg, scene.make_rays(cfg, fx["pixels"]))
+    out = _forward(net, cfg, scene.make_rays(cfg, fx["pixels"], bg_color=bg))
     assert np.abs(out["coarse_raycolor"][0].detach().cpu().numpy() - fx["coarse_raycolor"]).max() <= 1e-4
     assert np.abs(out["weight"][0].cpu().numpy() - fx["weight"]).max() <= 1e-5
     assert np.abs(out["conf_coefficient"][0].detach().cpu().numpy() - fx["conf_coefficient"]).max() <= 1e-6

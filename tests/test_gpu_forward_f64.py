@@ -24,9 +24,13 @@ Bounds per (kernel, quantity), 4-5x the largest error measured over this file's 
 The BF16x3 paths carry the split's ~1e-5 (h-bar is stored as bf16 hi + lo, ~2^-17 of each value); the largest sigma errors are at
 alpha_bias -6 (softplus's exponential tail).  tests/test_forward_f64_oracle.py shows
 defects that pass the 1e-4 rule and fail a per-sample check of this kind.
+Section E (background, raydist_mode_unit 0, point values of a trained checkpoint; same card) stays inside this table, embeddings x10
+included, except composite / aux at alpha_bias 48 in mode 0 (2.5e-5 / 1.2e-5 measured, bounds set in that test).  In mode 0 the one
+choice float64 and fp32 can take differently is rd < 1e-8, which march takes in fp32 like the unit mode's.
 """
 import ctypes as C
 
+import numpy as np
 import pytest
 import torch
 
@@ -42,11 +46,13 @@ BOUNDS = {
     "general": dict(sigma=2e-5, rgb=7e-6, hbar=6e-5, composite=1e-5, aux=1e-5),
     "fp32": dict(sigma=3e-6, rgb=6e-7, composite=1e-5, aux=1e-5),
 }
+# point values beyond the table's (test_checkpoint_value_ranges): the entries of a kernel's row that differ there
+VALUE_BOUNDS = {}
 KERNELS = {"frozen": dict(), "general": dict(pnb_frozen=0), "fp32": dict(pnb_precision="fp32")}
 
 
 def _forward(net, rays):
-    r = {k: v.to(DEV) for k, v in rays.items()}
+    r = {k: (None if v is None else v.to(DEV)) for k, v in rays.items()}
     with torch.no_grad():
         out = net(r["campos"], r["raydir"], bg_color=r["bg_color"], camrotc2w=r["camrotc2w"], pixel_idx=r["pixel_idx"],
                   near=r["near"], far=r["far"], h=r["h"], w=r["w"], intrinsic=r["intrinsic"])
@@ -91,7 +97,9 @@ def _pre_errors(net, F):
 
 
 def _run(cfg_name, side=20, F=32, kernel="frozen", frames=False, order=2, rotated=True, alpha_bias=3.0, pixels=None, edit=None,
-         **over):
+         bg=(1.0, 1.0, 1.0), bounds=None, **over):
+    """bg: the background's three channels, or None (forward(bg_color=None): black).  over: options of harness.make_opt, e.g.
+    raydist_mode_unit=0.  bounds: entries of the kernel's BOUNDS row replaced for this case."""
     cfg = scene.CONFIGS[cfg_name]
     net, pts, opt = harness.build_model(cfg, DEV, alpha_bias=alpha_bias, seed=2, feat_dim=F, agg_intrp_order=order, **KERNELS[kernel],
                                         **over)
@@ -101,7 +109,11 @@ def _run(cfg_name, side=20, F=32, kernel="frozen", frames=False, order=2, rotate
         Rw = scene.edit_frames(pts["xyz"])
         npn.Rw2c = torch.nn.Parameter(Rw.to(DEV), requires_grad=False)
     rays = scene.make_rays(cfg, scene.centre_patch(cfg, side) if pixels is None else pixels,
-                           camrotc2w=scene.orbit_rotation() if rotated else None)
+                           camrotc2w=scene.orbit_rotation() if rotated else None, bg_color=bg or (0.0, 0.0, 0.0))
+    bg64 = rays["bg_color"][0].double()
+    if bg is None:
+        rays["bg_color"] = None
+    mode_unit = opt.raydist_mode_unit
     if edit is not None:
         edit(net, rays)
     out = _forward(net, rays)
@@ -126,8 +138,8 @@ def _run(cfg_name, side=20, F=32, kernel="frozen", frames=False, order=2, rotate
     mlp64 = {k: v.double() for k, v in harness.mlp_cpu(net.aggregator).items()}
     pidx, loc_w = ex["sample_pidx"].cpu(), ex["sample_loc_w"].cpu()
     shade = shade_oracle_rw2c.shade if frames else shade_oracle.shade
-    sh = shade(pts64, mlp64, pidx, loc_w, rays["raydir"][0][hit], campos, cam, opt.vsize, torch.ones(3), dtype=torch.float64,
-               agg_intrp_order=order)
+    sh = shade(pts64, mlp64, pidx, loc_w, rays["raydir"][0][hit], campos, cam, opt.vsize, bg64, dtype=torch.float64,
+               agg_intrp_order=order, raydist_mode_unit=mode_unit)
     errs = forward_check.sample_errors(got, sh, smap["srow"])
     ray_errs = {}
     if kernel == "frozen":
@@ -136,7 +148,7 @@ def _run(cfg_name, side=20, F=32, kernel="frozen", frames=False, order=2, rotate
     Rn, SR = pidx.shape[0], q.SR
     dec = torch.zeros(Rn * SR, 4, dtype=torch.float64)
     dec[smap["srow"]] = sr.double()
-    m = forward_check.march(dec.view(Rn, SR, 4), sh["ray_valid"], loc_w, campos, cam, opt.vsize, torch.ones(3))
+    m = forward_check.march(dec.view(Rn, SR, 4), sh["ray_valid"], loc_w, campos, cam, opt.vsize, bg64, raydist_mode_unit=mode_unit)
     col, op, bg = out["coarse_raycolor"][0].cpu(), out["coarse_point_opacity"][0].cpu(), out["coarse_is_background"][0].cpu()
     ray_errs["composite"] = torch.stack([(col - m["ray_color"]).abs().amax(-1), (op - m["opacity"]).abs().amax(-1),
                                          (bg - m["bg_T"]).abs().amax(-1)], -1).amax(-1)
@@ -144,7 +156,7 @@ def _run(cfg_name, side=20, F=32, kernel="frozen", frames=False, order=2, rotate
                                    (out["conf_coefficient"][0].cpu() - sh["conf_coefficient"]).abs().amax((-1, -2)),
                                    (out["blend_weight"][0].cpu() - m["blend_weight"]).abs().amax((-1, -2))], -1).amax(-1)
     # end to end: the float64 oracle's (sigma, rgb), composited with the raydist_mode_unit choice taken in fp32, as the reference takes it
-    m64 = forward_check.march(sh["decoded"], sh["ray_valid"], loc_w, campos, cam, opt.vsize, torch.ones(3))
+    m64 = forward_check.march(sh["decoded"], sh["ray_valid"], loc_w, campos, cam, opt.vsize, bg64, raydist_mode_unit=mode_unit)
     e2e = max((col - m64["ray_color"]).abs().max().item(), (op - m64["opacity"]).abs().max().item(),
               (bg - m64["bg_T"]).abs().max().item())
     # NaN in the buffers, the same call: equal bits
@@ -154,10 +166,14 @@ def _run(cfg_name, side=20, F=32, kernel="frozen", frames=False, order=2, rotate
     # every comparison first (the report), then the bounds
     rep = {k: forward_check.worst(e) for k, e in list(errs.items()) + list(ray_errs.items())}
     n_bg = float(sh["bg_T"].min())
-    print("\n[fwd-f64] %s side=%d F=%d %s frames=%d order=%d rot=%d ab=%g %s: R'=%d S=%d tiles=%d min bg_T=%.3f %s e2e=%.2e%s" % (
-        cfg_name, side, F, kernel, frames, order, rotated, alpha_bias, over, Rn, S, (S + 127) // 128, n_bg,
-        " ".join("%s=%.2e" % (k, v[0]) for k, v in rep.items()), e2e, " POISONED=%s" % poisoned if poisoned else ""))
-    b = BOUNDS[kernel]
+    # steps above 2 vsize_z (raydist_mode_unit 0 keeps them) and samples whose opacity is 1 in fp32
+    n_long, n_sat = int((m["ray_dist"] > 2 * float(opt.vsize[2])).sum()), int((op == 1).sum())
+    print("\n[fwd-f64] %s side=%d F=%d %s frames=%d order=%d rot=%d ab=%g bg=%s edit=%s %s: R'=%d of %d S=%d tiles=%d min bg_T=%.3g long=%d "
+          "o==1: %d %s e2e=%.2e%s" % (
+              cfg_name, side, F, kernel, frames, order, rotated, alpha_bias, bg, getattr(edit, "__name__", edit), over, Rn, hit.numel(), S,
+              (S + 127) // 128, n_bg, n_long, n_sat, " ".join("%s=%.2e" % (k, v[0]) for k, v in rep.items()), e2e,
+              " POISONED=%s" % poisoned if poisoned else ""))
+    b = dict(BOUNDS[kernel], **(bounds or {}))
     forward_check.check(errs, {k: b[k] for k in errs}, lambda i: forward_check.describe_sample(smap, i))
     forward_check.check({k: v for k, v in ray_errs.items() if k != "pre"}, b, lambda i: "ray row %d" % i)
     if "pre" in ray_errs:
@@ -165,7 +181,7 @@ def _run(cfg_name, side=20, F=32, kernel="frozen", frames=False, order=2, rotate
         forward_check.check(dict(pre=ray_errs["pre"]), b, lambda i: "point %d (block %d of %d points)" % (i, i // NP, NP))
     assert e2e <= TOL, "end to end: %.3e > %.0e" % (e2e, TOL)
     assert not poisoned, "outputs differ after NaN in the shading buffers: %s" % poisoned
-    smap["sample_pidx"] = pidx
+    smap.update(sample_pidx=pidx, hit=hit, n_long=n_long, n_sat=n_sat, rays=rays, out=out)
     return net, sh, smap
 
 
@@ -220,17 +236,6 @@ def test_alpha_bias_extremes(kernel, alpha_bias):
     _run("tiny", 20, kernel=kernel, alpha_bias=alpha_bias)
 
 
-def _edit_conf(net, rays):
-    """5 % of points_conf outside the clamp (0.0001, 1): zero, negative, tiny positive, above 1."""
-    c = net.neural_points.points_conf
-    N = c.shape[1]
-    g = torch.Generator().manual_seed(7)
-    idx = torch.randperm(N, generator=g)[:N // 20]
-    vals = torch.tensor([0.0, -0.3, 5e-5, 1.7, 1.0 + 1e-3, -1e-6, 9.99e-5, 30.0])
-    with torch.no_grad():
-        c[0, idx.to(c.device), 0] = vals.repeat(len(idx) // len(vals) + 1)[:len(idx)].to(c.device)
-
-
 def _edit_point_on_sample(net, rays):
     """One point moved exactly onto a sample position of a valid sample it neighbours: the 1e-6 clamp of the distance norm."""
     _forward(net, rays)
@@ -247,7 +252,7 @@ def _edit_point_on_sample(net, rays):
 @pytest.mark.parametrize("kernel", ["frozen", "general", "fp32"])
 @pytest.mark.parametrize("what", ["conf", "point_on_sample"])
 def test_value_edges(kernel, what):
-    edit = dict(conf=_edit_conf, point_on_sample=_edit_point_on_sample)[what]
+    edit = dict(conf=forward_check.edit_conf, point_on_sample=_edit_point_on_sample)[what]
     net, sh, smap = _run("tiny", 20, kernel=kernel, edit=edit)
     if what == "point_on_sample":
         assert float(sh["weight"].max()) > 0.999, "no pair at distance below the clamp"
@@ -255,3 +260,63 @@ def test_value_edges(kernel, what):
         pidx = smap["sample_pidx"]
         c = net.neural_points.points_conf[0, :, 0].detach().cpu()[pidx[pidx >= 0].long()]
         assert float(c.min()) < 0 and float(c.max()) > 1, "no pair reaches the clamp of conf_coefficient"
+
+
+# ---- E. the background, raydist_mode_unit 0, and point values of a trained checkpoint
+def _limb_patch(cfg, side):
+    """A patch across the limb of the shell: rays that hit it and rays that miss it."""
+    return scene.centre_patch(cfg, side) + np.float32([side // 2, 0])
+
+
+@pytest.mark.parametrize("kernel", ["frozen", "general", "fp32"])
+@pytest.mark.parametrize("bg", [(0.9, 0.1, 0.4), (0.0, 0.0, 0.0), None], ids=["coloured", "black", "none"])
+def test_background(kernel, bg):
+    """Three different channels (a channel of bg_color used for another shows), black, and forward(bg_color=None); render_full paints
+    the rays that miss the cloud with the background bit for bit."""
+    cfg = scene.CONFIGS["tiny"]
+    net, sh, smap = _run("tiny", 20, kernel=kernel, pixels=_limb_patch(cfg, 20), bg=bg)
+    hit, rays = smap["hit"], smap["rays"]
+    assert 0 < int(hit.sum()) < hit.numel(), "the patch needs rays that hit and rays that miss"
+    assert 0.05 < float(sh["bg_T"].min()) and float(sh["bg_T"].max()) > 0.5, "the background does not reach the hit rays' colour"
+    bgl = list(bg or (0.0, 0.0, 0.0))
+    with torch.no_grad():
+        full = net.render_full(rays["campos"][0].tolist(), rays["raydir"].to(DEV), rays["camrotc2w"][0], cfg.near, cfg.far, bgl)
+    net.check_errors()
+    assert torch.equal(full["ray_mask"][0].cpu() > 0, hit)
+    miss = ~hit
+    assert torch.equal(full["coarse_raycolor"][0].cpu()[miss], torch.tensor(bgl, dtype=torch.float32).expand(int(miss.sum()), 3))
+    assert bool((full["coarse_is_background"][0].cpu()[miss] == 1).all()) and bool((full["coarse_point_opacity"][0].cpu()[miss] == 0).all())
+    for k in ("coarse_raycolor", "coarse_point_opacity", "coarse_is_background"):       # and on the hit rays it is forward()'s result
+        assert torch.equal(full[k][0][hit.to(DEV)], smap["out"][k][0]), k
+
+
+@pytest.mark.parametrize("F,alpha_bias", [(32, 3.0), (63, 3.0), (32, 8.0), (32, 48.0)])
+@pytest.mark.parametrize("kernel", ["frozen", "general", "fp32"])
+def test_raydist_mode_unit_0(kernel, F, alpha_bias):
+    """The reference's default ray distances: the step from the shell's front crossing to its back crossing stays (~30 voxels, SR 80
+    reaches the back).  alpha_bias 48: sigma times that step is beyond fp32's 1 - exp(-x) < 1, so those samples have opacity 1 and the
+    transmittance behind them starts from the 1e-10 floor."""
+    # at alpha_bias 48 sigma reaches ~45, and the fp32 rounding of a step between depths of ~4 (a few 1e-7) times sigma moves an
+    # opacity by ~1e-5: composite and blend_weight are held to 4x what that case measured (2.5e-5, 1.2e-5) instead of the table's 1e-5
+    bounds = dict(composite=1e-4, aux=5e-5) if alpha_bias == 48.0 else None
+    _, sh, smap = _run("tiny", 16, F=F, kernel=kernel, alpha_bias=alpha_bias, SR=80, raydist_mode_unit=0, bg=(0.9, 0.1, 0.4), bounds=bounds)
+    assert smap["n_long"] > 100 and float(sh["ray_dist"].max()) > 20 * 0.03, "no step above 2 vsize_z: the case is the unit mode's"
+    if alpha_bias == 48.0:
+        assert smap["n_sat"] > 50, "no sample with opacity 1"
+
+
+@pytest.mark.parametrize("kernel", ["frozen", "general", "fp32"])
+@pytest.mark.parametrize("what", ["embedding_x4", "embedding_x10", "dir", "color"])
+def test_checkpoint_value_ranges(kernel, what):
+    """Embeddings of several units (PE arguments 4 f of tens of radians), non-unit and zero points_dir, colours outside [0, 1]."""
+    edit = dict(embedding_x4=forward_check.edit_embedding(4.0), embedding_x10=forward_check.edit_embedding(10.0),
+                dir=forward_check.edit_dir, color=forward_check.edit_color)[what]
+    net, sh, smap = _run("tiny", 20, kernel=kernel, edit=edit, bounds=VALUE_BOUNDS.get((what, kernel)))
+    npn = net.neural_points
+    if what == "dir":
+        n = npn.points_dir[0].norm(dim=-1)
+        assert int((n == 0).sum()) > 0 and float(n.max()) > 2.5
+    elif what == "color":
+        assert float(npn.points_color.min()) < -0.4 and float(npn.points_color.max()) > 1.4
+    else:
+        assert float(npn.points_embeding.abs().max()) > (6.0 if what == "embedding_x4" else 15.0)

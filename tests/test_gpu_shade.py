@@ -58,17 +58,20 @@ def test_render_matches_oracle(name, side, alpha_bias, over, precision):
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
-@pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1"])
+@pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1", "tiny_raydist0_bg"])
 def test_forward_matches_reference_fixture(name, golden_dir, precision):
     """The drop-in NeuralPointsRayMarching.forward() output dict vs what the reference module itself returned
-    (tiny_order1: the reference run with --agg_intrp_order 1, SURVEY 8(f) rank 4)."""
+    (tiny_order1: the reference run with --agg_intrp_order 1, SURVEY 8(f) rank 4; tiny_raydist0_bg: with --raydist_mode_unit 0 and
+    bg_color (0.9, 0.1, 0.4))."""
     fx = golden.load(golden_dir, name)
     cfg = scene.CONFIGS["tiny"]
     order = int(fx["agg_intrp_order"]) if "agg_intrp_order" in fx.files else 2
-    net, pts, opt = harness.build_model(cfg, DEV, SR=int(fx["SR"]), max_o=100000, agg_intrp_order=order, **_prec(precision))
+    mode_unit = int(fx["raydist_mode_unit"]) if "raydist_mode_unit" in fx.files else 1
+    net, pts, opt = harness.build_model(cfg, DEV, SR=int(fx["SR"]), max_o=100000, agg_intrp_order=order, raydist_mode_unit=mode_unit,
+                                        **_prec(precision))
     sd = {k[4:]: torch.from_numpy(fx[k]) for k in fx.files if k.startswith("mlp.")}
     net.aggregator.load_state_dict(sd)
-    rays = scene.make_rays(cfg, fx["pixels"])
+    rays = scene.make_rays(cfg, fx["pixels"], bg_color=fx["bg_color"].tolist() if "bg_color" in fx.files else (1.0, 1.0, 1.0))
     r = {k: v.to(DEV) for k, v in rays.items()}
     with torch.no_grad():
         out = net(r["campos"], r["raydir"], bg_color=r["bg_color"], camrotc2w=r["camrotc2w"], pixel_idx=r["pixel_idx"],

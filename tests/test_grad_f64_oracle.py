@@ -2,7 +2,8 @@
 float64 autograd run with the fp32 run's own LeakyReLU masks (`slopes=`): with the masks shared, every point and every MLP tensor agrees
 to ~1e-6 of scale, while against float64 with its own masks a few units flip sign and move their pairs' gradients by up to ~2e-3.
 A perturbation of a single point by 1e-5 of scale fails the strict comparison, and passes the bounded-outlier rule the other gradient
-tests use."""
+tests use.  Defects in the backward's use of bg_color and in its read of conf_coefficient's gradient that a white background and the
+constant 1e-3 hide fail under (0.9, 0.1, 0.4) and seeded random weights."""
 import numpy as np
 import pytest
 import torch
@@ -113,3 +114,43 @@ def test_a_one_point_error_is_caught(golden_dir, name, monkeypatch):
     bad["conf"][0, 1, 0] += 1e-5 * g64m["conf"][0, 1:].abs().max()
     with pytest.raises(AssertionError, match="points_conf"):
         _check_all(bad, g64m, n0)
+
+
+@pytest.mark.parametrize("defect", ["bg_taken_as_1", "bg_channels_0_2_swapped", "cc_gradient_strides_swapped"])
+def test_backward_defects_need_a_coloured_background_and_varying_conf_weights(golden_dir, defect):
+    """Injected into the oracle's backward: the suffix of the composite backward started from gR + gG + gB instead of g . bg_color (the
+    background left out of it), from g . bg_color with channels 0 and 2 swapped, and the gradient of conf_coefficient [R',SR,K] read
+    with the SR and K strides swapped.  With a white background and the constant weight 1e-3 every gradient agrees; with
+    (0.9, 0.1, 0.4) and a seeded random weight per entry the strict comparison fails."""
+    fx = golden.load(golden_dir, "tiny_opaque")
+    cfg = scene.CONFIGS["tiny"]
+    pts = scene.make_points(cfg)
+    rays = scene.make_rays(cfg, fx["pixels"])
+    mask = torch.from_numpy(fx["ray_mask"]) > 0
+    pidx = torch.from_numpy(fx["sample_pidx"])
+    Rn, SR, K = pidx.shape
+    n0 = int((np.clip(fx["sample_pidx"], 0, None) == 0).sum())
+    mlp = {k[4:]: torch.from_numpy(fx[k]) for k in fx.files if k.startswith("mlp.")}
+    for new_input in (False, True):
+        bg = torch.tensor([0.9, 0.1, 0.4]) if new_input else torch.ones(3)
+        w = 2e-3 * torch.rand(Rn, SR, K, generator=torch.Generator().manual_seed(9)) if new_input else torch.full((Rn, SR, K), 1e-3)
+        pts_g = {k: v.clone().requires_grad_(k in ("embedding", "conf")) for k, v in pts.items()}
+        sh = shade_oracle.shade(pts_g, mlp, pidx, torch.from_numpy(fx["sample_loc_w"]), rays["raydir"][0][mask], torch.tensor(cfg.campos),
+                                torch.eye(3), [cfg.vsize] * 3, bg)
+        T = sh["bg_T"] - sh["bg_T"].detach()          # zero, with bg_T's gradient
+        color = dict(bg_taken_as_1=sh["ray_color"] + T * (1 - bg), bg_channels_0_2_swapped=sh["ray_color"] + T * (bg.flip(0) - bg),
+                     cc_gradient_strides_swapped=sh["ray_color"])[defect]
+        w_bad = w.reshape(Rn, K, SR).transpose(1, 2) if defect == "cc_gradient_strides_swapped" else w
+        leaves = (pts_g["embedding"], pts_g["conf"])
+        ref = torch.autograd.grad((sh["ray_color"] ** 2).sum() + (sh["conf_coefficient"] * w).sum(), leaves, retain_graph=True)
+        bad = torch.autograd.grad((color ** 2).sum() + (sh["conf_coefficient"] * w_bad).sum(), leaves)
+
+        def check():
+            grad_check.check_points(bad[0], ref[0], "embedding", RTOL)
+            grad_check.check_conf(bad[1], ref[1], n0, RTOL)
+
+        if new_input:
+            with pytest.raises(AssertionError, match="points_conf" if defect == "cc_gradient_strides_swapped" else "embedding"):
+                check()
+        else:
+            check()

@@ -16,10 +16,14 @@ def _mlp_from(fx, prefix="mlp."):
     return {k[len(prefix):]: torch.from_numpy(fx[k]) for k in fx.files if k.startswith(prefix)}
 
 
-@pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1"])
+@pytest.mark.parametrize("name", ["tiny_opaque", "tiny_thin_sr8", "tiny_order1", "tiny_raydist0_bg"])
 def test_shade_oracle_matches_reference_fixture(name, golden_dir):
+    """tiny_raydist0_bg: the reference run with --raydist_mode_unit 0 and bg_color (0.9, 0.1, 0.4)."""
     fx = golden.load(golden_dir, name)
     order = int(fx["agg_intrp_order"]) if "agg_intrp_order" in fx.files else 2
+    mode_unit = int(fx["raydist_mode_unit"]) if "raydist_mode_unit" in fx.files else 1
+    bg = torch.from_numpy(fx["bg_color"]) if "bg_color" in fx.files else torch.ones(3)
+    assert (name == "tiny_raydist0_bg") == (mode_unit == 0 and len(set(bg.tolist())) == 3)
     cfg = scene.CONFIGS["tiny"]
     pts = scene.make_points(cfg)
     rays = scene.make_rays(cfg, fx["pixels"])
@@ -27,8 +31,13 @@ def test_shade_oracle_matches_reference_fixture(name, golden_dir):
     pts_g = {k: v.clone().requires_grad_(k in ("embedding", "color", "dir", "conf")) for k, v in pts.items()}
     mlp = {k: v.clone().requires_grad_(True) for k, v in _mlp_from(fx).items()}
     sh = shade_oracle.shade(pts_g, mlp, torch.from_numpy(fx["sample_pidx"]), torch.from_numpy(fx["sample_loc_w"]),
-                            rays["raydir"][0][mask], torch.tensor(cfg.campos), torch.eye(3), [cfg.vsize] * 3, torch.ones(3),
-                            agg_intrp_order=order)
+                            rays["raydir"][0][mask], torch.tensor(cfg.campos), torch.eye(3), [cfg.vsize] * 3, bg,
+                            agg_intrp_order=order, raydist_mode_unit=mode_unit)
+    if mode_unit == 0:      # the fixture has steps the unit mode would replace, and the two modes differ on it
+        assert float(sh["ray_dist"].max()) > 2 * cfg.vsize
+        unit = shade_oracle.shade(pts, mlp, torch.from_numpy(fx["sample_pidx"]), torch.from_numpy(fx["sample_loc_w"]), rays["raydir"][0][mask],
+                                  torch.tensor(cfg.campos), torch.eye(3), [cfg.vsize] * 3, bg, agg_intrp_order=order)
+        assert np.abs(unit["ray_color"].detach().numpy() - fx["coarse_raycolor"]).max() > 1e-2
     # forward: same torch build, same op order -> tight
     for a, b in (("ray_color", "coarse_raycolor"), ("opacity", "coarse_point_opacity"), ("weight", "weight"),
                  ("conf_coefficient", "conf_coefficient"), ("sample_loc", "sample_loc")):
