@@ -204,6 +204,9 @@ class TrainStep:
         loss = self.gradients(fwd_kwargs, gt, mark=mark).clone()
         self.opt_mlp.step()
         self.opt_pts.step()
+        # the fused Adam kernels write the parameters without advancing their autograd version, which is what the module's weight
+        # packs and its frozen per-point table are keyed on: advance it here, or the next call would shade with the old weights
+        torch.autograd.graph.increment_version(self.mlp_params + self.pt_params)
         (mark or (lambda name: None))("adam")
         if self.world > 1:
             dist.all_reduce(loss, op=dist.ReduceOp.SUM, group=self.group)

@@ -15,6 +15,7 @@ value raises NotImplementedError (no silent fallback).
 """
 import math
 import os
+import weakref
 
 import torch
 import torch.nn as nn
@@ -135,11 +136,18 @@ class PointAggregator(nn.Module):
         return {k: sd[k] for k in sd}
 
 
+def _same_objects(refs, tensors):
+    """True when the weak references `refs` point at exactly these tensor objects.  A cache key of (data_ptr, _version) alone also
+    matches a NEW tensor that the caching allocator placed where a freed one was (both at version 0)."""
+    return refs is not None and len(refs) == len(tensors) and all(r() is t for r, t in zip(refs, tensors))
+
+
 class MlpPack:
-    """W^T (zero padded) buffers for the kernels, refreshed when any parameter's version changes."""
+    """W^T (zero padded) buffers for the kernels, refreshed when any parameter's version changes or another tensor takes its place."""
 
     def __init__(self):
         self.key = None
+        self.src = None      # weak references to the 18 parameters the buffers were filled from (weights, then biases)
         self.wt = None
         self.bias = None
         self.desc = None
@@ -151,15 +159,18 @@ class MlpPack:
         ws = [sd[k + ".weight"] for k in MLP_KEYS]
         bs = [sd[k + ".bias"] for k in MLP_KEYS]
         key = tuple((t.data_ptr(), t._version) for t in ws + bs)
-        if key != self.key:
+        if key != self.key or not _same_objects(self.src, ws + bs):
             F = feat_dim_of_block1(ws[0].shape[1])
-            self.wt, self.bias = [], []
-            for w, b, shp, kp in zip(ws, bs, mlp_shapes(F), mlp_kpad(F)):
+            # a training step changes every weight: refill the padded buffers in place (their padding rows stay zero)
+            refill = self.wt is not None and self.wt[0].device == ws[0].device and self.wt[0].shape[0] == mlp_kpad(F)[0]
+            wts, self.bias = [], []
+            for i, (w, b, shp, kp) in enumerate(zip(ws, bs, mlp_shapes(F), mlp_kpad(F))):
                 assert tuple(w.shape) == shp, "MLP tensor shape %s != %s" % (tuple(w.shape), shp)
-                wt = torch.zeros((kp, shp[0]), dtype=torch.float32, device=w.device)
+                wt = self.wt[i] if refill else torch.zeros((kp, shp[0]), dtype=torch.float32, device=w.device)
                 wt[:shp[1]].copy_(w.detach().t())
-                self.wt.append(wt.contiguous())
+                wts.append(wt)
                 self.bias.append(b.detach().contiguous().float())
+            self.wt = wts
             d = _lib.Mlp()
             for i in range(9):
                 d.w[i] = self.wt[i].data_ptr()
@@ -167,6 +178,7 @@ class MlpPack:
             d.feat_dim = F
             self.desc = d
             self.key = key
+            self.src = [weakref.ref(t) for t in ws + bs]
             self.key_l1 = (key[0], key[9])
             lib = _lib.load()
             nb = lib.pnb_mlp_pack_bytes(F)
@@ -215,14 +227,15 @@ def points_desc_of(npnts):
 
 
 def rw2c_host_of(npnts):
-    """Rw2c as 9 host floats, cached on the module per tensor version (one tiny D2H copy when it changes)."""
+    """Rw2c as 9 host floats, cached on the module per tensor and version (one tiny D2H copy when it changes)."""
     R = npnts.Rw2c
     if R is None:
         return None
     key = (R.data_ptr(), R._version)
-    if getattr(npnts, "_pnb_rw2c_key", None) != key:
+    if getattr(npnts, "_pnb_rw2c_key", None) != key or not _same_objects(getattr(npnts, "_pnb_rw2c_src", None), (R,)):
         npnts._pnb_rw2c_host = _to_list(R)
         npnts._pnb_rw2c_key = key
+        npnts._pnb_rw2c_src = (weakref.ref(R),)
     return npnts._pnb_rw2c_host
 
 
@@ -475,6 +488,7 @@ def _init_state(mod):
     mod._generation = 0
     mod._pre = None              # hoisted layer-1 table of the frozen pipeline + the versions it was computed from
     mod._pre_key = None
+    mod._pre_src = None          # weak references to points_embeding, block1.0 weight and bias of the table
     mod._valid_per_ray = 0.0     # densest call seen so far (valid samples per ray): sizes the shading workspace
     mod._status_pending = []     # (event, pinned [err, query counters], R) of render_full() calls not yet checked
     mod._status_free = []
@@ -525,10 +539,12 @@ class NeuralPointsRayMarching(nn.Module):
 
     # -------------------------------------------------------------------------------------------------
     def _point_pre(self, mlp_desc, pts_desc, stream):
-        """Hoisted layer-1 table of the frozen pipeline (pnb_point_pre), rebuilt when points_embeding or block1.0 changed."""
+        """Hoisted layer-1 table of the frozen pipeline (pnb_point_pre), rebuilt when points_embeding or block1.0 changed (version)
+        or were replaced by other tensors.  `self._pre_key = None` forces a rebuild."""
         emb = self.neural_points.points_embeding
         key = (emb.data_ptr(), emb._version, emb.shape[1], self._mlp.key_l1)
-        if key != self._pre_key:
+        srcs = (emb, self._mlp.src[0](), self._mlp.src[len(MLP_KEYS)]())
+        if key != self._pre_key or not _same_objects(getattr(self, "_pre_src", None), srcs):
             lib = _lib.load()
             nb = lib.pnb_point_pre_bytes(int(pts_desc.N))
             if self._pre is None or self._pre.numel() * 4 < nb or self._pre.device != emb.device:
@@ -536,6 +552,7 @@ class NeuralPointsRayMarching(nn.Module):
             _lib.check(lib.pnb_point_pre(_lib.C.byref(pts_desc), _lib.C.byref(mlp_desc), self._pre.data_ptr(), self._pre.numel() * 4,
                                          stream), "pnb_point_pre")
             self._pre_key = key
+            self._pre_src = [weakref.ref(t) for t in srcs]
         return self._pre
 
     def _poll_status(self, block=False):

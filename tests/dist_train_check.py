@@ -4,10 +4,12 @@
 Checks of the multi-GPU paths on real GPUs (SURVEY 8e):
   1. optimisation: parallel.TrainStep, each rank on ITS rays of the step -> the exchanged gradient equals - to fp32 summation order - the
      gradient of the un-sharded step on the union of the rays (run by every rank on a second copy of the model), and after k Adam steps the
-     replicas are BIT-identical on every rank (identical all-reduced gradients + identical Adam);
+     replicas are BIT-identical on every rank (identical all-reduced gradients + identical Adam), and each rank's module renders what a
+     module loaded from its own state dict renders (its weight packs and frozen table follow the fused Adam's writes);
   2. render: one frame interleave-sharded over the ranks + all-gather == the frame rendered by one rank, bit for bit;
   3. grow: every rank probes its own frames, allgather_new_points, grow_points -> identical clouds, grid rebuilt, render still agrees.
 Prints one JSON line on rank 0; exit code != 0 on any failure."""
+import copy
 import json
 import os
 import sys
@@ -17,7 +19,7 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from pointnerf_b200 import harness, parallel, scene  # noqa: E402
+from pointnerf_b200 import checkpoint, harness, parallel, point_query, scene  # noqa: E402
 
 
 def fwd_kwargs(cfg, pixels, dev):
@@ -79,6 +81,17 @@ def main():
         alls = [torch.empty_like(flat) for _ in range(world)]
         dist.all_gather(alls, flat)
         assert all(torch.equal(alls[0], a) for a in alls), "replicas differ across ranks (sparse=%s)" % sparse
+        # a TrainStep compared with a TrainStep cannot see weights the module failed to refresh: compare with a module loaded from the state
+        loaded = checkpoint.load_checkpoint({k: v.detach().clone() for k, v in net.state_dict().items()}, copy.copy(net.opt), dev)
+        rd = scene.make_rays(cfg, scene.centre_patch(cfg, 100))["raydir"][0].to(dev)
+        t = point_query.host_t_table(cfg.near, cfg.far, cfg.D).to(dev)
+        with torch.no_grad():
+            got, want = (m.render_full(list(cfg.campos), rd, torch.eye(3), cfg.near, cfg.far, [1., 1., 1.], t=t) for m in (net, loaded))
+        net.check_errors()
+        loaded.check_errors()
+        differs = [k for k in got if not torch.equal(got[k], want[k])]
+        assert not differs, "rank %d (sparse=%s): render_full after the steps differs from a module loaded from the state dict in %s" % (
+            rank, sparse, differs)
         moved = (flat - torch.cat([p.detach().reshape(-1) for p in harness.build_model(cfg, dev, alpha_bias=3.0)[0].parameters()])).abs().max().item()
         assert moved > 1e-3
         err = gerr

@@ -139,6 +139,25 @@ def _train_worker(rank, world, port, sparse, ret):
         dist.destroy_process_group()
 
 
+def test_fused_adam_step_advances_parameter_versions(monkeypatch):
+    """torch's fused Adam (what TrainStep builds on CUDA) writes the parameters without advancing their autograd version, which keys the
+    module's weight packs and frozen per-point table: TrainStep.step advances it itself.  CPU fused Adam stands in for the CUDA one."""
+    adam = torch.optim.Adam
+    monkeypatch.setattr(parallel.torch.optim, "Adam", lambda params, **kw: adam(params, **dict(kw, fused=True)))
+    net = _StubNet()
+    ts = parallel.TrainStep(net)
+    assert ts.opt_mlp.defaults["fused"] and ts.opt_pts.defaults["fused"]
+    params = ts.mlp_params + ts.pt_params
+    R = 31
+    gt = torch.rand(R, 3, generator=torch.Generator().manual_seed(11))
+    for it in range(2):
+        before = [(p.detach().clone(), p._version) for p in params]
+        ts.step(dict(ray_ids=(torch.arange(R) * 5 + it) % 97), gt)
+        for p, (b, v) in zip(params, before):
+            assert not torch.equal(p.detach(), b), "the step did not move a parameter"
+            assert p._version > v, "a parameter moved without advancing its version"
+
+
 def test_world2_gloo_train_step_matches_unsharded_and_replicas_identical():
     for sparse in (False, True):
         mgr = mp.Manager()

@@ -6,58 +6,16 @@ valid_list / samp_off / pair_off, the masks are handed to oracle/shade_oracle.py
 of the 18 MLP tensors must agree with float64 autograd within one bound per backward mode (oracle/grad_check.py), with no allowance
 for outliers: a bug that touches a few pair rows only (a partial GEMM tile, one split-K slab, one K slot, a channel edge of the
 F = 63 scatter) shows.  Each case reports how many units the kernel's masks flip against float64's own."""
-import ctypes as C
-
 import pytest
 import torch
 
 from oracle import forward_check, grad_check, shade_oracle, shade_oracle_rw2c
-from pointnerf_b200 import harness, lib, scene
+from pointnerf_b200 import harness, scene
 from pointnerf_b200.point_query import make_cam_opts
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-# (points, MLP tensors): the largest error allowed, relative to the tensor's scale, per (pnb_bwd_fp32 mode, pnb_precision), 4-5x the
-# largest measured over this file's cases on an H100 80GB HBM3 at a 400 W power limit:
-#   mode 0 (BF16x3 recompute, dX, dW)    bf16x3: points 8.9e-6, MLP 2.8e-5    fp32: points 8.3e-6, MLP 2.7e-5
-#   mode 4 (fp32 recompute, BF16x3 dX/dW) bf16x3: points 8.8e-6, MLP 2.6e-5
-#   mode 1 (fp32 CUDA-core GEMMs)         bf16x3: points 4.7e-6, MLP 1.2e-6    fp32: points 4.9e-7, MLP 6.7e-7
-# The cases below the rotated-camera ones (background, raydist_mode_unit 0, saturated rays, random conf_coefficient weights, frozen groups,
-# checkpoint value ranges; H100 80GB HBM3 at 700 W) measured at most: tensor-core modes points 1.3e-5, MLP 2.8e-5; mode 1 points 5.5e-6,
-# MLP 3.5e-6 (both in raydist_mode_unit 0 at SR 80).
-# The tensor-core dX / dW GEMMs carry the ~1e-5 of the BF16x3 split (tests/test_gpu_umma.py); in mode 1 the points see the BF16x3
-# forward's (sigma, rgb), from which the composite backward starts.  One flipped or lost pair row moves its points by ~1e-3 of scale.
-RTOL = {(0, "bf16x3"): (4e-5, 1.2e-4), (0, "fp32"): (4e-5, 1.2e-4), (4, "bf16x3"): (4e-5, 1.2e-4),
-        (1, "bf16x3"): (2e-5, 5e-6), (1, "fp32"): (2e-6, 3e-6)}
-
-
-def _kernel_masks(net, q, F, camrotc2w):
-    """The backward's masks as `slopes=` of the oracle (pair rows in the flattened [R',SR,K] order of sample_pidx >= 0, colour rows per
-    sample slot), the dense export of the query, and the pair-row count."""
-    l = lib.load()
-    S, P = int(q.counters["n_valid"]), int(q.counters["n_pairs"])
-    out = (C.c_void_p * 10)()
-    ws = net._bwd_ws
-    lib.check(l.pnb_backward_tables(ws.data_ptr(), ws.numel(), S, q.desc.cap_samples, F, out), "pnb_backward_tables")
-    dev_view = forward_check.dev_view
-    H = [dev_view(ws, out[0], torch.float32, (P, 256)), dev_view(ws, out[1], torch.float32, (P, 272))[:, :256],
-         dev_view(ws, out[2], torch.float32, (P, 256)), dev_view(ws, out[3], torch.float32, (P, 256))]
-    Cc = [dev_view(ws, out[i], torch.float32, (S, 128)) for i in (4, 5, 6)]
-    pair_off = dev_view(ws, out[7], torch.int32, (S + 1,)).long()
-    row_samp = dev_view(ws, out[8], torch.int32, (P,)).long()
-    pidx = dev_view(ws, out[9], torch.int32, (P,)).long()
-    ex = q.export(make_cam_opts(list(q.desc.campos), camrotc2w), want_pers=False, want_dirs=False)
-    SR = q.SR
-    # valid sample -> (ray, sample slot) -> its row of the export; pair row -> (its sample, K slot)
-    srow = forward_check.sample_map(q, ex)["srow"]
-    flat = forward_check.pair_map(dict(srow=srow), pair_off, row_samp, pidx, ex, q.K)
-    order = torch.argsort(flat)
-    slopes = [torch.where(h[order] > 0, 1.0, 0.01).double() for h in H]
-    for c in Cc:
-        s = torch.ones(ex["sample_pidx"].shape[0] * SR, 128, dtype=torch.float64)
-        s[srow] = torch.where(c > 0, 1.0, 0.01).double()
-        slopes.append(s)
-    return slopes, ex, P
+RTOL = grad_check.RTOL       # the bound of each backward mode, measured over this file's cases
 
 
 def _forward(net, rays):
@@ -118,7 +76,7 @@ def _run_case(cfg_name, side, F=32, frames=False, order=2, mode=0, precision="bf
           cc_weights).backward()
     net.check_errors()
     q = net.last
-    slopes, ex, P = _kernel_masks(net, q, F, cam)
+    slopes, ex, P = grad_check.kernel_masks(net, q, F, cam)
     hit = ex["ray_mask"].cpu() > 0
     # float64 autograd through the oracle with the kernel's masks, on the kernel's own sample geometry
     pts_g = dict(xyz=npn.xyz.detach().cpu().double(), Rw2c=R.double())
