@@ -198,6 +198,18 @@ int pnb_aux_outputs(const pnb_query_t* q, const pnb_points_t* pts, const long lo
  * straight-through estimator, every entry adds its gradient to the conf of its (clamped-to-0) point index. */
 int pnb_aux_conf_backward(const pnb_query_t* q, const long long* d_rows, int n_rows,
                           const float* d_grad_conf_coefficient, float* d_grad_conf, pnb_stream_t stream);
+/* Probe outputs of point growing (opt.prob == 1, models/neural_points_volumetric_model.py:331-351) from the compacted query and the
+ * [R,SR] opacity of pnb_composite_forward: per ray the first slot of maximal opacity oi (torch.max's tie rule; slots past nsamp have
+ * opacity 0), its opacity max_opacity [n], its position max_loc [n,3] (bit-identical to pnb_query_export's sample_loc_w; 0 past
+ * nsamp), far_dist [n] = min over the K slots of |xyz[max(pidx,0)] - loc| (an empty slot measures point 0, as the reference's clamped
+ * gather), and avg_{color [n,3], dir [n,3], conf [n], emb [n,F]} = sum_k w_k attr[max(pidx_k,0)] in k order with
+ * w_k = weight * conf_coefficient at oi (bit-identical to the product of pnb_aux_outputs' two outputs; 0 for an empty slot).
+ * d_rows: the R' hit rays (int64 ray ids, ascending; n = n_rows), or NULL for all rays (n_rows must be R; a ray that missed gets zeros
+ * everywhere, as the reference's unmask fills it).  d_slot (int32 [n]) and d_weight ([n,K]) are optional copies of oi and w_k.
+ * K > PNB_MAX_K, SR > PNB_MAX_SR or a width without an instantiation: PNB_ERR_UNSUPPORTED. */
+int pnb_probe_outputs(const pnb_query_t* q, const pnb_points_t* pts, const long long* d_rows, int n_rows, const float* d_opacity,
+                      float* d_max_opacity, float* d_max_loc, float* d_far_dist, float* d_avg_color, float* d_avg_dir,
+                      float* d_avg_conf, float* d_avg_emb, int32_t* d_slot, float* d_weight, pnb_stream_t stream);
 
 /* ---- shading forward on the tensor cores (wgmma, BF16x3 error-compensated split) ---- */
 /* Packs block1 / block3 / colour-branch weights of a pnb_mlp_t (fp32 W^T buffers) into wgmma operand images (hi/lo bf16, one

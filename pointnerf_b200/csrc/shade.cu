@@ -392,6 +392,123 @@ __global__ void __launch_bounds__(128) k_aux_conf_bwd(AuxParams p) {
     if ((threadIdx.x & 31) == 0 && g0 != 0.f) atomicAdd(&p.grad_conf[0], g0);
 }
 
+// ------------------------------------------------------------------------------------------ probe outputs (point growing)
+// The opt.prob == 1 outputs of neural_points_volumetric_model.py:331-351, straight from the compacted query and the [R, SR] opacity
+// of k_composite: one warp per ray.
+//   arg-max slot oi   torch.max(opacity, -1): the first maximal slot wins a tie; slots past nsamp hold opacity 0
+//   position          the sample at oi as pnb_query_export writes it (slot_t / ray_pos; 0 past nsamp)
+//   weights           w_k = weight_k * conf_coefficient_k at oi, formed as k_aux_outputs forms both factors (same bits)
+//   far_dist          min over the K slots of |xyz[max(pidx_k, 0)] - loc|: an empty slot measures point 0 (the reference's clamp)
+//   averages          sum_k w_k * attr[max(pidx_k, 0)] in k order, lanes over the 7 + F channels (colour, dir, conf, embedding)
+// rows: the R' hit rays (compacted outputs), or NULL for all R rays (full-R outputs, zeros for a ray that missed, as unmask fills
+// them, :120-131).  Per-point frames play no part.
+struct ProbeParams {
+    pnb_query_t q;
+    pnb_points_t pts;
+    const long long* rows;     // [n_rows] ray ids, ascending, or NULL (row = ray)
+    int n_rows;
+    const float* opacity;      // [R, SR]
+    float* max_opacity;        // [n_rows]
+    float* max_loc;            // [n_rows, 3]
+    float* far_dist;           // [n_rows]
+    float* avg_color;          // [n_rows, 3]
+    float* avg_dir;            // [n_rows, 3]
+    float* avg_conf;           // [n_rows]
+    float* avg_emb;            // [n_rows, F]
+    int32_t* slot;             // [n_rows] or NULL (tests): oi
+    float* weight;             // [n_rows, K] or NULL (tests): w_k
+};
+
+template <int F>
+__global__ void __launch_bounds__(128) k_probe_outputs(ProbeParams p) {
+    const pnb_query_t& q = p.q;
+    const int SR = q.SR, K = q.K, lane = threadIdx.x & 31;
+    const long long rr = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (rr >= p.n_rows) return;
+    const int r = p.rows ? (int)p.rows[rr] : (int)rr;
+    constexpr int NC = 7 + F;   // colour 3, dir 3, conf 1, embedding F
+    if (!p.rows && !q.ray_hit[r]) {
+        for (int c = lane; c < NC; c += 32) {
+            if (c < 3) p.avg_color[rr * 3 + c] = 0.f;
+            else if (c < 6) p.avg_dir[rr * 3 + c - 3] = 0.f;
+            else if (c == 6) p.avg_conf[rr] = 0.f;
+            else p.avg_emb[rr * F + c - 7] = 0.f;
+        }
+        if (lane < 3) p.max_loc[rr * 3 + lane] = 0.f;
+        if (lane == 0) { p.max_opacity[rr] = 0.f; p.far_dist[rr] = 0.f; if (p.slot) p.slot[rr] = 0; }
+        if (p.weight && lane < K) p.weight[rr * K + lane] = 0.f;
+        return;
+    }
+    // first maximum: ascending slots within a lane keep the first (strict >), the butterfly keeps the lower slot of equal values
+    const float* op = p.opacity + (size_t)r * SR;
+    float best = -INFINITY;
+    int bj = SR;
+    for (int j = lane; j < SR; j += 32) {
+        const float v = op[j];
+        if (v > best) { best = v; bj = j; }
+    }
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) {
+        const float v = __shfl_xor_sync(0xffffffffu, best, d);
+        const int j = __shfl_xor_sync(0xffffffffu, bj, d);
+        if (v > best || (v == best && j < bj)) { best = v; bj = j; }
+    }
+    const int oi = bj;
+    const int n = q.nsamp[r];
+    float3 l = make_float3(0.f, 0.f, 0.f);
+    const int32_t* pid = nullptr;
+    if (oi < n) {
+        l = ray_pos(q, ray_dir(q, r), slot_t(q, r, oi));
+        pid = q.cand_pidx + (size_t)(q.samp_off[r] + oi) * K;
+    }
+    // the K weights and distances, every lane the same (K <= 8 points): k_aux_outputs' expressions in its k order
+    const float c_first = conf_coef(__ldg(p.pts.conf));
+    float w[PNB_MAX_K], c[PNB_MAX_K];
+    int pi[PNB_MAX_K];
+    float wsum = 0.f, far = INFINITY;
+#pragma unroll
+    for (int k = 0; k < PNB_MAX_K; ++k) {
+        if (k >= K) break;
+        const int pk = pid ? pid[k] : -1;
+        pi[k] = max(pk, 0);
+        const float dx = __ldg(&p.pts.xyz[3 * pi[k]]) - l.x, dy = __ldg(&p.pts.xyz[3 * pi[k] + 1]) - l.y,
+                    dz = __ldg(&p.pts.xyz[3 * pi[k] + 2]) - l.z;
+        w[k] = pk >= 0 ? inv_dist_weight(dx, dy, dz) : 0.f;
+        c[k] = pk >= 0 ? conf_coef(__ldg(&p.pts.conf[pk])) : c_first;
+        wsum += w[k];
+        far = fminf(far, sqrtf(dx * dx + dy * dy + dz * dz));
+    }
+#pragma unroll
+    for (int k = 0; k < PNB_MAX_K; ++k) {
+        if (k >= K) break;
+        w[k] = __fmul_rn(norm_weight(w[k], wsum), c[k]);
+    }
+    // lanes over channels: products rounded, then summed in k order (no contraction)
+    for (int ch = lane; ch < NC; ch += 32) {
+        float s = 0.f;
+#pragma unroll
+        for (int k = 0; k < PNB_MAX_K; ++k) {
+            if (k >= K) break;
+            const float a = ch < 3 ? __ldg(&p.pts.color[3 * pi[k] + ch])
+                          : ch < 6 ? __ldg(&p.pts.dir[3 * pi[k] + ch - 3])
+                          : ch == 6 ? __ldg(&p.pts.conf[pi[k]])
+                          : __ldg(&p.pts.emb[(size_t)pi[k] * F + ch - 7]);
+            s = __fadd_rn(s, __fmul_rn(a, w[k]));
+        }
+        if (ch < 3) p.avg_color[rr * 3 + ch] = s;
+        else if (ch < 6) p.avg_dir[rr * 3 + ch - 3] = s;
+        else if (ch == 6) p.avg_conf[rr] = s;
+        else p.avg_emb[rr * F + ch - 7] = s;
+    }
+    if (lane < 3) p.max_loc[rr * 3 + lane] = lane == 0 ? l.x : lane == 1 ? l.y : l.z;
+    if (lane == 0) { p.max_opacity[rr] = best; p.far_dist[rr] = far; if (p.slot) p.slot[rr] = oi; }
+    if (p.weight) {
+#pragma unroll
+        for (int k = 0; k < PNB_MAX_K; ++k)
+            if (k < K && lane == k) p.weight[rr * K + k] = w[k];
+    }
+}
+
 }  // namespace pnb
 
 using namespace pnb;
@@ -461,6 +578,29 @@ extern "C" int pnb_aux_outputs(const pnb_query_t* q, const pnb_points_t* pts, co
     p.weight = d_weight; p.cc = d_conf_coefficient; p.blend = d_blend_weight; p.grad_cc = nullptr; p.grad_conf = nullptr;
     const long long n = (long long)n_rows * q->SR;
     k_aux_outputs<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(p);
+    PNB_CHECK_CUDA(cudaGetLastError());
+    return PNB_OK;
+}
+
+extern "C" int pnb_probe_outputs(const pnb_query_t* q, const pnb_points_t* pts, const long long* d_rows, int n_rows, const float* d_opacity,
+                                 float* d_max_opacity, float* d_max_loc, float* d_far_dist, float* d_avg_color, float* d_avg_dir,
+                                 float* d_avg_conf, float* d_avg_emb, int32_t* d_slot, float* d_weight, pnb_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PNB_REQUIRE(q && pts && d_opacity && d_max_opacity && d_max_loc && d_far_dist && d_avg_color && d_avg_dir && d_avg_conf && d_avg_emb,
+                PNB_ERR_INVALID, "pnb_probe_outputs: null argument");
+    PNB_REQUIRE(q->K >= 1 && q->K <= PNB_MAX_K, PNB_ERR_UNSUPPORTED, "pnb_probe_outputs: K=%d unsupported", q->K);
+    PNB_REQUIRE(q->SR >= 1 && q->SR <= PNB_MAX_SR, PNB_ERR_UNSUPPORTED, "pnb_probe_outputs: SR=%d unsupported (1..%d)", q->SR, PNB_MAX_SR);
+    int F = 0;
+    { const int rc = feat_check(pts, nullptr, "pnb_probe_outputs", &F); if (rc) return rc; }
+    PNB_REQUIRE(d_rows || n_rows == q->R, PNB_ERR_INVALID, "pnb_probe_outputs: without a row list n_rows must be R (%d), got %d", q->R, n_rows);
+    if (n_rows <= 0) return PNB_OK;
+    ProbeParams p;
+    p.q = *q; p.pts = *pts; p.rows = d_rows; p.n_rows = n_rows; p.opacity = d_opacity;
+    p.max_opacity = d_max_opacity; p.max_loc = d_max_loc; p.far_dist = d_far_dist; p.avg_color = d_avg_color; p.avg_dir = d_avg_dir;
+    p.avg_conf = d_avg_conf; p.avg_emb = d_avg_emb; p.slot = d_slot; p.weight = d_weight;
+    const unsigned blocks = (unsigned)((n_rows + 3) / 4);   // 4 rays (warps) per block
+    if (F == PNB_FEAT) k_probe_outputs<PNB_FEAT><<<blocks, 128, 0, stream>>>(p);
+    else k_probe_outputs<PNB_FEAT_DTU><<<blocks, 128, 0, stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }

@@ -473,6 +473,34 @@ class _AuxFn(torch.autograd.Function):
         return None, None, None, None, g_conf
 
 
+def probe_keys(F):
+    """(key, channels) of the probe outputs (opt.prob == 1, neural_points_volumetric_model.py:331-351), in pnb_probe_outputs' order."""
+    return (("ray_max_shading_opacity", 1), ("ray_max_sample_loc_w", 3), ("ray_max_far_dist", 1), ("shading_avg_color", 3),
+            ("shading_avg_dir", 3), ("shading_avg_conf", 1), ("shading_avg_embedding", F))
+
+
+def probe_outputs(mod, q, opacity, rows=None, diag=False):
+    """The probe outputs of one query (pnb_probe_outputs): dict key -> [n, C] for the hit rays `rows` (int64 ray ids, ascending) or,
+    with rows None, for all R rays (zeros where a ray missed).  opacity: the [R, SR] opacity of the same call.  diag: also "slot"
+    (int32 [n], the arg-max slot) and "weight" ([n, K], weight * conf_coefficient at that slot)."""
+    lib = _lib.load()
+    npnts = mod.neural_points
+    dev = opacity.device
+    n = q.R if rows is None else int(rows.shape[0])
+    out = {k: torch.empty((n, c), dtype=torch.float32, device=dev) for k, c in probe_keys(int(npnts.points_embeding.shape[-1]))}
+    slot = torch.empty((n,), dtype=torch.int32, device=dev) if diag else None
+    weight = torch.empty((n, int(q.desc.K)), dtype=torch.float32, device=dev) if diag else None
+    if n == 0:
+        return dict(out, slot=slot, weight=weight) if diag else out
+    opacity = opacity.detach().contiguous()
+    pts = points_desc_of(npnts)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    _lib.check(lib.pnb_probe_outputs(_lib.C.byref(q.desc), _lib.C.byref(pts), ptr(rows), n, opacity.data_ptr(),
+                                     *[t.data_ptr() for t in out.values()], ptr(slot), ptr(weight), stream), "pnb_probe_outputs")
+    return dict(out, slot=slot, weight=weight) if diag else out
+
+
 def _init_state(mod):
     """Per-module launch state (weight packs, workspaces).  Works on our module and on the reference's
     NeuralPointsRayMarching after install_into()."""
@@ -685,15 +713,20 @@ class NeuralPointsRayMarching(nn.Module):
         ev.record(torch.cuda.current_stream(dev))
         self._status_pending.append((ev, host, q.R))
 
-    def render_full(self, campos, raydir, camrotc2w, near, far, bg_color, t=None):
+    def render_full(self, campos, raydir, camrotc2w, near, far, bg_color, t=None, probe=False):
         """Full-R outputs, fill_invalid semantics, no host sync: dict(coarse_raycolor [1,R,3],
         coarse_point_opacity [1,R,SR], coarse_is_background [1,R,1], ray_mask [1,R]).  No gradients (frozen-cloud pipeline).
+        probe=True: also the seven probe outputs of point growing (probe_keys, [1,R,C]; zeros where a ray missed, as the reference's
+        unmask fills them), one more kernel on the same query.
         The device status of the call (workspace overflow, time-out) is copied to pinned memory behind the kernels and raised
-        by a LATER call or by check_errors(); runner.render_image checks it before returning."""
+        by a LATER call or by check_errors(); runner.render_image / probe_image check it before returning."""
         q, ray_color, opacity, bg_T, ray_mask = self._run(campos, raydir, camrotc2w, near, far, bg_color, False, t=t, frozen=True)
+        out = dict(coarse_raycolor=ray_color[None], coarse_point_opacity=opacity[None],
+                   coarse_is_background=bg_T[None, :, None], ray_mask=ray_mask[None])
+        if probe:
+            out.update({k: v[None] for k, v in probe_outputs(self, q, opacity).items()})
         self._queue_status(q, ray_color.device)
-        return dict(coarse_raycolor=ray_color[None], coarse_point_opacity=opacity[None],
-                    coarse_is_background=bg_T[None, :, None], ray_mask=ray_mask[None])
+        return out
 
     def forward(self, campos, raydir, gt_image=None, bg_color=None, camrotc2w=None, pixel_idx=None, near=None,
                 far=None, focal=None, h=None, w=None, intrinsic=None, **kargs):
@@ -733,7 +766,7 @@ class NeuralPointsRayMarching(nn.Module):
         opt = self.opt
         want_aux = (getattr(opt, "sparse_loss_weight", 0) > 0) or ("conf_coefficient" in getattr(opt, "zero_one_loss_items", [])) \
             or getattr(opt, "prob", 0) != 0                       # point_aggregators.py:812-813
-        if want_aux and inds.shape[0] > 0 and getattr(opt, "prob", 0) != 1:
+        if want_aux and inds.shape[0] > 0:
             # weight / conf_coefficient / blend_weight of the reference dict (:325-329): one kernel on the compacted query
             # blend_weight is detached (as in the reference), so the kernel's opacity input carries no graph: a loss on conf_coefficient
             # alone must not reach the shading backward
@@ -741,44 +774,10 @@ class NeuralPointsRayMarching(nn.Module):
             out["weight"] = wgt[None]
             out["blend_weight"] = blend[None, ..., None]
             out["conf_coefficient"] = conf_coefficient[None]
-        elif want_aux and inds.shape[0] > 0:
-            # probe pass (opt.prob == 1, point growing): the same three outputs with eager torch ops on the dense export, which the
-            # probe outputs below need anyway
-            cam = make_cam_opts(_to_list(campos)[:3], _to_list(camrotc2w)[:9])
-            ex = q.export(cam, want_pers=False, want_dirs=False)
-            pidx = ex["sample_pidx"]
-            mask = pidx >= 0
-            idx = pidx.clamp(min=0).long()
-            d = npnts.xyz.detach()[idx] - ex["sample_loc_w"][:, :, None, :]
-            wgt = mask * (1.0 / torch.clamp(torch.norm(d, dim=-1), min=1e-6))
-            wgt = wgt / torch.clamp(torch.sum(wgt, dim=-1, keepdim=True), min=1e-8)
-            # index_select (as the reference, neural_points.py:717): its backward is one index_add_, not a sort-based scatter
-            c0 = torch.index_select(npnts.points_conf[0, :, 0], 0, idx.reshape(-1)).view(idx.shape)
-            conf_coefficient = c0 - (c0 - torch.clamp(c0, min=0.0001, max=1)).detach()
-            op = out["coarse_point_opacity"][0].detach()
-            acc = torch.cumprod(1. - op + 1e-10, dim=-1)
-            acc_T = torch.cat([torch.ones_like(acc[:, :1]), acc[:, :-1]], dim=-1)
-            out["weight"] = wgt[None].detach()
-            out["blend_weight"] = (op * acc_T)[None, ..., None]
-            out["conf_coefficient"] = conf_coefficient[None]
             if getattr(opt, "prob", 0) == 1:
-                # probe outputs for point growing (neural_points_volumetric_model.py:331-351), same torch ops on the
-                # dense export: arg-max-opacity sample of every ray and the weighted average of its neighbours
-                K = pidx.shape[-1]
-                omax, oind = torch.max(out["coarse_point_opacity"], dim=-1, keepdim=True)          # [1,R',1]
-                out["ray_max_shading_opacity"] = omax
-                oi = oind[0, :, 0]
-                rows = torch.arange(pidx.shape[0], device=pidx.device)
-                loc_max = ex["sample_loc_w"][rows, oi]                                                # [R',3]
-                out["ray_max_sample_loc_w"] = loc_max[None]
-                wsel = (wgt * conf_coefficient.detach())[rows, oi][..., None]                         # [R',K,1]
-                idx_max = idx[rows, oi]                                                               # [R',K] (clamped, :707)
-                xyz_max = npnts.xyz.detach()[idx_max]
-                out["ray_max_far_dist"] = torch.min(torch.norm(xyz_max - loc_max[:, None, :], dim=-1), dim=-1, keepdim=True)[0][None]
-                out["shading_avg_color"] = torch.sum(npnts.points_color.detach()[0][idx_max] * wsel, dim=-2)[None]
-                out["shading_avg_dir"] = torch.sum(npnts.points_dir.detach()[0][idx_max] * wsel, dim=-2)[None]
-                out["shading_avg_conf"] = torch.sum(npnts.points_conf.detach()[0][idx_max] * wsel, dim=-2)[None]
-                out["shading_avg_embedding"] = torch.sum(npnts.points_embeding.detach()[0][idx_max] * wsel, dim=-2)[None]
+                # probe outputs for point growing (:331-351): arg-max-opacity sample of every ray and the weighted average of its
+                # neighbours, one kernel on the same rows
+                out.update({k: v[None] for k, v in probe_outputs(self, q, opacity, inds).items()})
         elif getattr(opt, "prob", 0) == 1:
             dev = ray_color.device                                                                    # :352-361
             out.update({"ray_max_shading_opacity": torch.zeros([0, 0, 1, 1], device=dev), "ray_max_sample_loc_w": torch.zeros([0, 0, 3], device=dev),
