@@ -110,6 +110,12 @@ typedef struct {
     const float* t;          /* borrowed */
     int32_t t_ray_stride;
     float campos[3];
+    /* Explicit sample geometry of the perspective-frustum query (pnb_frustum_samples; all NULL for the world query, whose samples lie
+     * at campos + raydir * t): the querier's [R',SR,3] tensors, borrowed.  Every slot of a hit ray is a candidate there, so candidate
+     * s of ray r is row samp_off[r] / SR = ray_rank[r], slot s - samp_off[r], of these tensors. */
+    const float* xs_loc_w;   /* world position of every slot (sample_loc_w) */
+    const float* xs_loc;     /* perspective position x/z, y/z, z, jitter applied (sample_loc): dists[3..5] and the ray distances */
+    const float* xs_dir;     /* view direction of every slot (sample_ray_dirs) */
 } pnb_query_t;
 
 /* Camera + scalar options of the shading / compositing stage. */
@@ -185,6 +191,11 @@ int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, const pnb_m
 int pnb_composite_forward(const pnb_query_t* q, const pnb_shade_opts_t* opts, const float* d_sigma_rgb,
                           float* d_ray_color, float* d_opacity, float* d_bg_T, int8_t* d_ray_mask,
                           pnb_stream_t stream);
+/* The same with a per-ray background bg_ray [R,3] (bgmodel plane: the reference composites without a background colour and
+ * fill_invalid adds coarse_is_background * bg_ray, models/neural_points_volumetric_model.py:101-103, :294-295): ray_color is
+ * bg_T * bg_ray + colour for a hit ray (product and sum rounded in that order) and bg_ray for a miss.  opts->bg_color is not read. */
+int pnb_composite_forward_bg_ray(const pnb_query_t* q, const pnb_shade_opts_t* opts, const float* d_sigma_rgb, const float* d_bg_ray,
+                                 float* d_ray_color, float* d_opacity, float* d_bg_T, int8_t* d_ray_mask, pnb_stream_t stream);
 
 /* ---- auxiliary training outputs ----
  * `weight` [R',SR,K], `conf_coefficient` [R',SR,K] and `blend_weight` [R',SR] of the reference's output dict
@@ -337,6 +348,17 @@ int pnb_frustum_query(const pnb_frustum_t* fr, const int32_t* d_pixel_idx, int R
 int pnb_frustum_export(const pnb_frustum_t* fr, const int32_t* d_pixel_idx, int R, const void* ws, size_t ws_bytes,
                        const int8_t* d_ray_mask, int R2, float radius_limit2, float depth_limit2, int32_t* d_pixel_idx_cur,
                        int32_t* d_sample_pidx, float* d_sample_loc, pnb_stream_t stream);
+/* Sample-compacted layout (pnb_query_t) of one frustum query for the shading, compositing, auxiliary, probe and backward entry points,
+ * which then read the explicit geometry of the querier's tuple instead of forming positions from raydir and t.  d_ray_mask [R] int8
+ * and R2 (its number of hit rays, on the host) come from pnb_frustum_query; d_sample_pidx [R2,SR,K] from pnb_frustum_export;
+ * d_sample_loc_w, d_sample_loc (jitter applied) and d_sample_ray_dirs [R2,SR,3] from the querier's pers2w.  The four tensors are
+ * borrowed and must outlive every call on q.  Every slot of a hit ray is a candidate sample (nsamp = SR): cand_pidx is
+ * d_sample_pidx itself, samp_nvalid counts its non-negative entries (they come first, canonical order), ray_hit is the ray mask
+ * (a hit ray may have no neighbour at all, as in the reference), and the counters are those of pnb_query.  Nothing synchronises. */
+size_t pnb_frustum_samples_bytes(int R, int R2, int SR);
+int pnb_frustum_samples(pnb_query_t* q, void* ws, size_t ws_bytes, const int8_t* d_ray_mask, int R, int R2, int SR, int K,
+                        const int32_t* d_sample_pidx, const float* d_sample_loc_w, const float* d_sample_loc,
+                        const float* d_sample_ray_dirs, pnb_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -261,7 +261,7 @@ __global__ void __launch_bounds__(256) k_bwd_counts(pnb_query_t q, int n_valid, 
 }
 // One warp per valid sample, 4 lanes per pair row: the fp32 forward's row builder, writing the dense block1 input, the block3 extras
 // and the view PE to the recompute buffers.
-template <bool PP, int F>
+template <bool PP, int F, bool XSAMP = false>
 __global__ void __launch_bounds__(256) k_bwd_build(BwdParams p) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= p.n_valid) return;
@@ -271,7 +271,7 @@ __global__ void __launch_bounds__(256) k_bwd_build(BwdParams p) {
     const long row = (long)p.pair_off[vi] + k;               // packed: only the sample's neighbours (its first slots) own a row
     float* cx = p.CX + (long)vi * 288;
     float* er = p.X3 + row * 272 + 256;
-    const Fp32Pair pr = fp32_pair<PP>(q, p.pts, p.o, true, s, min((int)q.samp_nvalid[s], q.K), lane, cx + 256);
+    const Fp32Pair pr = fp32_pair<PP, XSAMP>(q, p.pts, p.o, true, s, min((int)q.samp_nvalid[s], q.K), lane, cx + 256);
     if (lane < 8) cx[280 + lane] = 0.f;
     if (!pr.g.valid) return;
     if (part == 0) { p.wc[row] = pr.wc; p.wn[row] = pr.wn; p.pidx[row] = pr.pidx; p.row_samp[row] = vi; }
@@ -462,7 +462,7 @@ __global__ void __launch_bounds__(128) k_dw_small(const float* __restrict__ X, l
 }
 
 // Scatter to the points: embedding (through PE), colour, dir, conf.  4 lanes per pair row (8 embedding channels per lane, 16 for F = 63).
-template <bool PP, int F>
+template <bool PP, int F, bool XSAMP = false>
 __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* __restrict__ dwc, float* __restrict__ d_emb,
                                                      float* __restrict__ d_color, float* __restrict__ d_dir, float* __restrict__ d_conf) {
     constexpr int CPL = F == PNB_FEAT ? 8 : 16;
@@ -497,7 +497,7 @@ __global__ void __launch_bounds__(256) k_bwd_scatter(BwdParams p, const float* _
             // extras: (dir' - view')[3], <dir', view'>  with dir' = M_p dir (the point's frame) and view' in the frame of the sample's
             // slot-0 point  ->  d dir = M_p^T (g[3:6] + g[6] * view')
             const uint32_t s = p.q.valid_list[p.row_samp[row]];
-            const float3 ov = view_in_points<PP>(p.pts, p.o, view_point<PP>(p.q, s), ray_dir(p.q, cand_ray(p.q, s)));
+            const float3 ov = view_in_points<PP>(p.pts, p.o, view_point<PP>(p.q, s), cand_view_dir<XSAMP>(p.q, s));
             float gx = ge[3] + ge[6] * ov.x, gy = ge[4] + ge[6] * ov.y, gz = ge[5] + ge[6] * ov.z;
             float ox, oy, oz;
             rot3T(point_frame<PP>(p.pts, p.o, pi), gx, gy, gz, ox, oy, oz);
@@ -520,8 +520,8 @@ struct CompBwdParams {
 
 // EXT: the upstream gradients of opacity and bg_T (each optional, as is the colour's); without it the kernel reads d ray_color only.
 // With T_{j+1} = T_j (1 - o_j + 1e-10) and bg_T = T_end, the bg_T gradient enters the suffix beside g.bg, and the opacity gradient
-// adds to d o_j directly.
-template <bool EXT>
+// adds to d o_j directly.  XSAMP: explicit samples (pair_inputs.cuh).
+template <bool EXT, bool XSAMP = false>
 __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
     int r = blockIdx.x * blockDim.x + threadIdx.x;
     const pnb_query_t& q = p.q;
@@ -533,7 +533,7 @@ __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
         for (int j = 0; j < n; ++j) p.d_sigma_rgb[s0 + j] = make_float4(0.f, 0.f, 0.f, 0.f);
         return;
     }
-    const float3 dir = ray_dir(q, r);
+    const float3 dir = XSAMP ? make_float3(0.f, 0.f, 0.f) : ray_dir(q, r);
     const bool col = !EXT || p.d_ray_color;
     const float gR = col ? p.d_ray_color[3 * r] : 0.f, gG = col ? p.d_ray_color[3 * r + 1] : 0.f,
                 gB = col ? p.d_ray_color[3 * r + 2] : 0.f;
@@ -542,9 +542,9 @@ __global__ void __launch_bounds__(128) k_composite_bwd(CompBwdParams p) {
     float o_[PNB_MAX_SR], rd_[PNB_MAX_SR], T_[PNB_MAX_SR];
     float Tend;
     {
-        float cm = slot_depth(q, p.o, r, n, 0, dir), T = 1.0f;
+        float cm = slot_depth<XSAMP>(q, p.o, r, n, 0, dir), T = 1.0f;
         for (int j = 0; j < n; ++j) {
-            const float rd = ray_dist_step(q, p.o, r, n, j, dir, cm);
+            const float rd = ray_dist_step<XSAMP>(q, p.o, r, n, j, dir, cm);
             float o1 = 0.f;
             if (q.samp_nvalid[s0 + j] > 0) o1 = 1.0f - expf(-p.sigma_rgb[s0 + j].x * rd);
             o_[j] = o1; rd_[j] = rd; T_[j] = T;
@@ -648,8 +648,11 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     CompBwdParams cp;
     cp.q = *q; cp.o = *opts; cp.sigma_rgb = (const float4*)d_sigma_rgb_fwd; cp.d_ray_color = d_ray_color; cp.d_sigma_rgb = L.d_sigma_rgb;
     cp.d_opacity = d_opacity; cp.d_bg_T = d_bg_T;
-    if (d_ray_color && !d_opacity && !d_bg_T) k_composite_bwd<false><<<(q->R + 127) / 128, 128, 0, st>>>(cp);   // colour-only loss
-    else k_composite_bwd<true><<<(q->R + 127) / 128, 128, 0, st>>>(cp);
+    const bool xs = q->xs_loc_w != nullptr;                  // explicit samples (the frustum query)
+    { const int rc = xs_check(q, pts, F, "pnb_shade_backward"); if (rc) return rc; }
+    void (*comp)(CompBwdParams) = d_ray_color && !d_opacity && !d_bg_T ? (xs ? k_composite_bwd<false, true> : k_composite_bwd<false>)   // colour-only loss
+                                                                       : (xs ? k_composite_bwd<true, true> : k_composite_bwd<true>);
+    comp<<<(q->R + 127) / 128, 128, 0, st>>>(cp);
     if (n_valid <= 0) { PNB_CHECK_CUDA(cudaGetLastError()); return PNB_OK; }
     PNB_REQUIRE(n_pairs >= n_valid && n_pairs <= n_valid * PNB_MAX_K, PNB_ERR_INVALID, "pnb_shade_backward: n_pairs %d inconsistent with n_valid %d", n_pairs, n_valid);
     const int S = n_valid, P = n_pairs;      // pair-level buffers hold one row per VALID (sample, neighbour) pair
@@ -669,6 +672,7 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     const bool pp = pts->rw2c != nullptr;                    // per-point frames
     void (*build)(BwdParams) = F == PNB_FEAT ? (pp ? k_bwd_build<true, PNB_FEAT> : k_bwd_build<false, PNB_FEAT>)
                                              : (pp ? k_bwd_build<true, PNB_FEAT_DTU> : k_bwd_build<false, PNB_FEAT_DTU>);
+    if (xs) build = k_bwd_build<false, PNB_FEAT_DTU, true>;
     build<<<wb, 256, 0, st>>>(p);
     gemm_nn(cx, L.X1, KP1, mlp->w[0], 256, L.H1, 256, P, 256, KP1, mlp->b[0], 1);
     gemm_nn(cx, L.H1, 256, mlp->w[1], 256, L.X3, 272, P, 256, 256, mlp->b[1], 1);   // H2 into X3[:, :256]
@@ -719,6 +723,7 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     void (*scatter)(BwdParams, const float*, float*, float*, float*, float*) =
         F == PNB_FEAT ? (pp ? k_bwd_scatter<true, PNB_FEAT> : k_bwd_scatter<false, PNB_FEAT>)
                       : (pp ? k_bwd_scatter<true, PNB_FEAT_DTU> : k_bwd_scatter<false, PNB_FEAT_DTU>);
+    if (xs) scatter = k_bwd_scatter<false, PNB_FEAT_DTU, true>;
     scatter<<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;

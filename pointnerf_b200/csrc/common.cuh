@@ -48,6 +48,15 @@ static inline int feat_check(const pnb_points_t* pts, const pnb_mlp_t* mlp, cons
     *F = fp;
     return PNB_OK;
 }
+// Explicit samples (the frustum query, q->xs_loc_w set) are instantiated for the DTU scripts' configuration only: F = 63, one
+// uniform Rw2c, and all three geometry tensors given.  Sets the error text on failure.
+static inline int xs_check(const pnb_query_t* q, const pnb_points_t* pts, int F, const char* fn) {
+    if (!q->xs_loc_w) return PNB_OK;
+    PNB_REQUIRE(q->xs_loc && q->xs_dir, PNB_ERR_INVALID, "%s: explicit samples need xs_loc_w, xs_loc and xs_dir", fn);
+    PNB_REQUIRE(F == PNB_FEAT_DTU && !pts->rw2c, PNB_ERR_UNSUPPORTED,
+                "%s: the frustum query's samples are shaded with point_features_dim 63 and a uniform Rw2c only", fn);
+    return PNB_OK;
+}
 
 // Bump allocator over a caller-provided workspace.
 struct Carver {

@@ -255,12 +255,14 @@ static GridLayout carve_grid(void* buf, size_t cap, int N, const int32_t dim[3])
 
 using namespace pnb;
 
-extern "C" int pnb_version(void) { return 107; }   // 101: pnb_points_t.rw2c; 102: pnb_shade_backward takes d_opacity, d_bg_T;
+extern "C" int pnb_version(void) { return 108; }   // 101: pnb_points_t.rw2c; 102: pnb_shade_backward takes d_opacity, d_bg_T;
                                                    // 103: pnb_points_t / pnb_mlp_t.feat_dim (F = 32 | 63), F-sized *_bytes();
                                                    // 104: pnb_backward_tables (test-only: the backward's recompute buffers)
                                                    // 105: pnb_frustum_{bytes,build,query_bytes,query,export}, pnb_frustum_t (5)
                                                    // 106: pnb_shade_tc_buffers (test-only: the forward's h-bar and sigma)
                                                    // 107: pnb_probe_outputs (opt.prob == 1 outputs, compacted or full-R)
+                                                   // 108: pnb_query_t.xs_{loc_w,loc,dir} (explicit samples), pnb_frustum_samples{,_bytes},
+                                                   //      pnb_composite_forward_bg_ray
 extern "C" const char* pnb_last_error(void) { return pnb::g_err; }
 extern "C" size_t pnb_struct_size(int which) {
     switch (which) {

@@ -1,7 +1,7 @@
 // The reference's per-pair shading inputs, defined once for every kernel that builds or reads them: the fp32 forward
 // (k_shade_fwd), the tensor-core builders (k_shade_wg), the backward's recompute (k_bwd_build), and the kernels that need one
 // piece (k_color_wg, k_aux_outputs, k_composite, k_composite_bwd, k_bwd_scatter, k_bwd_reduce_fwd).
-//   sample position          diff_ray_marching.py:386
+//   sample position          diff_ray_marching.py:386 (world query); the frustum querier's tuple (XSAMP, below)
 //   point frames (Rw2c)      neural_points.py:717, point_aggregators.py:491-496 (uniform [3,3], or per point [N,3,3]: the pair's point
 //                            for dists and dir, the sample's slot-0 point for the view direction, :506, :526, :566)
 //   dists / linear weights   point_aggregators.py:727-814, :421-429 (conf_coefficient: neural_points.py:706-717, :722-724)
@@ -59,18 +59,46 @@ __device__ __forceinline__ float3 ray_pos(const pnb_query_t& q, float3 dir, floa
 }
 // the ray of candidate sample s (samp_ray = ray << 7 | slot)
 __device__ __forceinline__ int cand_ray(const pnb_query_t& q, uint32_t s) { return (int)(q.samp_ray[s] >> 7); }
+// Sample source, a compile-time parameter XSAMP of every helper and kernel that reads a sample's geometry.  World query (XSAMP false):
+// slot j of ray r lies at campos + raydir * t[steps], is seen along its ray's direction, and its perspective position is w2pers of
+// that.  Explicit samples (XSAMP true, the perspective-frustum query, pnb_frustum_samples): the querier's [R',SR,3] tensors give the
+// world position (sample_loc_w), the perspective position with its jitter (sample_loc) and the view direction (sample_ray_dirs) of
+// every slot (neural_points_volumetric_model.py:268-277, point_aggregators.py:773-781).  There every slot of a hit ray is a candidate,
+// so candidate s is entry s of those tensors, and slot j of ray r is entry samp_off[r] + j.
+__device__ __forceinline__ float3 ld_f3(const float* v, size_t i) { return make_float3(__ldg(&v[3 * i]), __ldg(&v[3 * i + 1]), __ldg(&v[3 * i + 2])); }
 struct CandSample {
-    float3 dir;   // its ray's direction
+    float3 dir;   // view direction: its ray's direction (XSAMP: the sample's own)
     float3 pos;   // world position
 };
+template <bool XSAMP = false>
 __device__ __forceinline__ CandSample cand_sample(const pnb_query_t& q, uint32_t s) {
+    CandSample c;
+    if (XSAMP) {
+        c.dir = ld_f3(q.xs_dir, s);
+        c.pos = ld_f3(q.xs_loc_w, s);
+        return c;
+    }
     const uint32_t rj = q.samp_ray[s];
     const int r = (int)(rj >> 7);
     const float t = slot_t(q, r, (int)(rj & 127u));
-    CandSample c;
     c.dir = ray_dir(q, r);
     c.pos = ray_pos(q, c.dir, t);
     return c;
+}
+// perspective position of candidate sample s for pair_geom: the querier's (XSAMP); the world query forms it from the world position there
+template <bool XSAMP = false>
+__device__ __forceinline__ float3 cand_pers(const pnb_query_t& q, uint32_t s) {
+    return XSAMP ? ld_f3(q.xs_loc, s) : make_float3(0.f, 0.f, 0.f);
+}
+// view direction of candidate sample s
+template <bool XSAMP = false>
+__device__ __forceinline__ float3 cand_view_dir(const pnb_query_t& q, uint32_t s) {
+    return XSAMP ? ld_f3(q.xs_dir, s) : ray_dir(q, cand_ray(q, s));
+}
+// world position of slot j < nsamp of ray r
+template <bool XSAMP = false>
+__device__ __forceinline__ float3 slot_pos(const pnb_query_t& q, int r, int j) {
+    return XSAMP ? ld_f3(q.xs_loc_w, q.samp_off[r] + j) : ray_pos(q, ray_dir(q, r), slot_t(q, r, j));
 }
 // ------------------------------------------------------------------------------------------ point frames
 // World -> canonical rotation of point pi, row-major (neural_points.Rw2c, gathered per neighbour: neural_points.py:717).  PP (per-point
@@ -114,8 +142,10 @@ struct PairGeom {
     float cc;        // conf_coefficient
     float dist[6];   // world offset + perspective terms (:782-784); the offset rotated into the point's frame
 };
-template <bool PP>
-__device__ __forceinline__ PairGeom pair_geom(const pnb_points_t& pts, const pnb_shade_opts_t& o, int pidx, float3 l) {
+// l: the sample's world position; lp (XSAMP): its perspective position, which the world query forms as w2pers(l)
+template <bool PP, bool XSAMP = false>
+__device__ __forceinline__ PairGeom pair_geom(const pnb_points_t& pts, const pnb_shade_opts_t& o, int pidx, float3 l,
+                                              float3 lp = make_float3(0.f, 0.f, 0.f)) {
     PairGeom g;
     g.valid = pidx >= 0;
     g.pi = g.valid ? pidx : 0;
@@ -123,7 +153,8 @@ __device__ __forceinline__ PairGeom pair_geom(const pnb_points_t& pts, const pnb
     const float dx = px - l.x, dy = py - l.y, dz = pz - l.z;
     float xpp, ypp, zpp, xsp, ysp, zsp;
     w2pers(o, px, py, pz, xpp, ypp, zpp);
-    w2pers(o, l.x, l.y, l.z, xsp, ysp, zsp);
+    if (XSAMP) { xsp = lp.x; ysp = lp.y; zsp = lp.z; }
+    else w2pers(o, l.x, l.y, l.z, xsp, ysp, zsp);
     g.dist[3] = xpp * zpp - xsp * zsp;
     g.dist[4] = ypp * zpp - ysp * zsp;
     g.dist[5] = zpp - zsp;
@@ -153,19 +184,23 @@ __device__ __forceinline__ float softplus_m1(float a) {
 __device__ __forceinline__ float raw2out_color(float x) { return 1.0f / (1.0f + expf(-x)) * (1.0f + 2.0f * 0.001f) - 0.001f; }
 
 // ------------------------------------------------------------------------------------------ ray distances
-// camera depth of slot j of ray r (n filled slots); an unfilled slot holds the world origin (SURVEY a17)
+// camera depth of slot j of ray r (n filled slots); an unfilled slot holds the world origin (SURVEY a17).  XSAMP: the z of the querier's
+// sample_loc, written for every slot (an empty one sits at near - vsize_z / 2, DESIGN.md §5 F6); dir is not read.
+template <bool XSAMP = false>
 __device__ __forceinline__ float slot_depth(const pnb_query_t& q, const pnb_shade_opts_t& o, int r, int n, int j, float3 dir) {
+    if (XSAMP) return __ldg(&q.xs_loc[3 * ((size_t)q.samp_off[r] + j) + 2]);
     if (j < n) return cam_depth(o, ray_pos(q, dir, slot_t(q, r, j)));
     return cam_depth(o, make_float3(0.f, 0.f, 0.f));
 }
 // Ray distance of slot j: the step of the cumulative maximum of the slot depths to slot j + 1 (vsize_z for the last slot), replaced
 // by vsize_z below 1e-8 or, with raydist_mode_unit, above 2 vsize_z.  cm: the cumulative maximum up to slot j (start: slot_depth
 // of slot 0), advanced to slot j + 1.
+template <bool XSAMP = false>
 __device__ __forceinline__ float ray_dist_step(const pnb_query_t& q, const pnb_shade_opts_t& o, int r, int n, int j, float3 dir, float& cm) {
     const float vz = o.vsize_z;
     float rd;
     if (j + 1 < q.SR) {
-        const float cmn = fmaxf(cm, slot_depth(q, o, r, n, j + 1, dir));
+        const float cmn = fmaxf(cm, slot_depth<XSAMP>(q, o, r, n, j + 1, dir));
         rd = cmn - cm;
         cm = cmn;
     } else {
@@ -194,16 +229,18 @@ struct Fp32Pair {
     float wc;     // weight * conf_coefficient (0 for an empty slot)
     float3 ov;    // view direction in the sample's view frame
 };
-template <bool PP>
+template <bool PP, bool XSAMP = false>
 __device__ __forceinline__ Fp32Pair fp32_pair(const pnb_query_t& q, const pnb_points_t& pts, const pnb_shade_opts_t& o, bool have,
                                               uint32_t s, int nk, int lane, float* vpe) {
     const int k = lane >> 2, part = lane & 3;   // neighbour slot, quarter of the feature vector
     CandSample cs = {};
+    float3 lp = make_float3(0.f, 0.f, 0.f);
     Fp32Pair r;
     r.pidx = -1;
     int p0 = 0;
     if (have) {
-        cs = cand_sample(q, s);
+        cs = cand_sample<XSAMP>(q, s);
+        if (XSAMP) lp = cand_pers<XSAMP>(q, s);
         if (k < nk) r.pidx = q.cand_pidx[(size_t)s * q.K + k];
         p0 = view_point<PP>(q, s);
     }
@@ -215,7 +252,7 @@ __device__ __forceinline__ Fp32Pair fp32_pair(const pnb_query_t& q, const pnb_po
         vpe[lane] = sn;
         vpe[12 + lane] = cn;
     }
-    r.g = pair_geom<PP>(pts, o, r.pidx, cs.pos);
+    r.g = pair_geom<PP, XSAMP>(pts, o, r.pidx, cs.pos, lp);
     float wsum = part == 0 ? r.g.w : 0.f;       // sum over the 8 slots
     for (int d = 16; d > 0; d >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, d);
     r.wn = norm_weight(r.g.w, wsum);

@@ -214,6 +214,37 @@ __global__ void __launch_bounds__(128) k_export(pnb_query_t q, float R00, float 
     }
 }
 
+// ------------------------------------------------------------------------------------------ frustum query -> compacted samples
+// pnb_frustum_samples: one thread per (ray, slot).  A hit ray lists all SR slots as candidates, row ray_rank[r] of the dense tensors,
+// so candidate s = ray_rank[r] * SR + j is entry s of [R',SR,...]; its neighbour count is the number of non-negative indices (the
+// frustum export writes them first).
+__global__ void __launch_bounds__(256) k_fs_rays(int R, int SR, const int8_t* __restrict__ ray_mask, int* __restrict__ nsamp,
+                                                 uint8_t* __restrict__ ray_hit) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= R) return;
+    const bool hit = ray_mask[r] != 0;
+    ray_hit[r] = hit ? 1 : 0;
+    nsamp[r] = hit ? SR : 0;
+}
+__global__ void __launch_bounds__(256) k_fs_samples(int R, int SR, int K, const uint8_t* __restrict__ ray_hit,
+                                                    const uint32_t* __restrict__ samp_off, const int32_t* __restrict__ pidx,
+                                                    uint32_t* __restrict__ samp_ray, uint8_t* __restrict__ samp_nvalid, int* counters) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    int nv = 0;
+    if (i < (long long)R * SR) {
+        const int r = (int)(i / SR), j = (int)(i - (long long)r * SR);
+        if (ray_hit[r]) {
+            const uint32_t s = samp_off[r] + j;
+            for (int k = 0; k < K; ++k) nv += pidx[(size_t)s * K + k] >= 0 ? 1 : 0;
+            samp_ray[s] = ((uint32_t)r << 7) | (uint32_t)j;
+            samp_nvalid[s] = (uint8_t)nv;
+        }
+    }
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) nv += __shfl_xor_sync(0xffffffffu, nv, d);
+    if ((threadIdx.x & 31) == 0 && nv) atomicAdd(&counters[PNB_QC_N_PAIRS], nv);
+}
+
 struct QueryLayout {
     int* nsamp;
     uint32_t* samp_off;
@@ -334,5 +365,53 @@ extern "C" int pnb_query_export(const pnb_query_t* q, const pnb_shade_opts_t* ca
                                                               q->ray_rank, d_ray_row, d_ray_mask, d_sample_pidx,
                                                               d_sample_loc_w, d_sample_loc, d_sample_ray_dirs);
     PNB_CHECK_CUDA(cudaGetLastError());
+    return PNB_OK;
+}
+
+// The per-candidate arrays of pnb_query over a frustum query's dense result (cand_pidx is not carved: the shading reads the
+// caller's [R2,SR,K] indices in place).
+extern "C" size_t pnb_frustum_samples_bytes(int R, int R2, int SR) {
+    return carve_query(nullptr, 0, R, SR, 0, R2 * SR).bytes;
+}
+
+extern "C" int pnb_frustum_samples(pnb_query_t* q, void* ws, size_t ws_bytes, const int8_t* d_ray_mask, int R, int R2, int SR, int K,
+                                   const int32_t* d_sample_pidx, const float* d_sample_loc_w, const float* d_sample_loc,
+                                   const float* d_sample_ray_dirs, pnb_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PNB_REQUIRE(q && ws && d_ray_mask && (R2 == 0 || (d_sample_pidx && d_sample_loc_w && d_sample_loc && d_sample_ray_dirs)),
+                PNB_ERR_INVALID, "pnb_frustum_samples: null argument");
+    PNB_REQUIRE(R > 0 && R < (1 << 25), PNB_ERR_INVALID, "pnb_frustum_samples: R=%d out of range [1, 2^25)", R);
+    PNB_REQUIRE(R2 >= 0 && R2 <= R, PNB_ERR_INVALID, "pnb_frustum_samples: R2=%d outside 0..R=%d", R2, R);
+    PNB_REQUIRE(K >= 1 && K <= PNB_MAX_K, PNB_ERR_UNSUPPORTED, "pnb_frustum_samples: K=%d unsupported", K);
+    PNB_REQUIRE(SR >= 1 && SR <= PNB_MAX_SR, PNB_ERR_UNSUPPORTED, "pnb_frustum_samples: SR=%d unsupported (1..%d)", SR, PNB_MAX_SR);
+    PNB_REQUIRE((long long)R * SR < (1ll << 31), PNB_ERR_UNSUPPORTED, "pnb_frustum_samples: R*SR too large");
+    const int cap = R2 * SR;
+    QueryLayout L = carve_query(ws, ws_bytes, R, SR, 0, cap);
+    PNB_REQUIRE(L.bytes <= ws_bytes, PNB_ERR_WORKSPACE, "pnb_frustum_samples: workspace %zu < required %zu", ws_bytes, L.bytes);
+    const uint32_t cs = (uint32_t)(cap > 0 ? cap : 1);
+    PNB_CHECK_CUDA(cudaMemsetAsync(L.counters, 0, 16 * sizeof(int), stream));
+    PNB_CHECK_CUDA(cudaMemsetAsync(L.samp_nvalid, 0, cs, stream));
+    k_fs_rays<<<(R + 255) / 256, 256, 0, stream>>>(R, SR, d_ray_mask, L.nsamp, L.ray_hit);
+    int rc = exclusive_scan_u32(L.nsamp, 3, L.samp_off, (uint32_t)R, L.scan_tmp, stream);
+    if (rc) return rc;
+    rc = exclusive_scan_u32(L.ray_hit, 2, L.ray_rank, (uint32_t)R, L.scan_tmp, stream);
+    if (rc) return rc;
+    const long long n = (long long)R * SR;
+    k_fs_samples<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(R, SR, K, L.ray_hit, L.samp_off, d_sample_pidx, L.samp_ray,
+                                                                  L.samp_nvalid, L.counters);
+    PNB_CHECK_CUDA(cudaGetLastError());
+    rc = exclusive_scan_u32(L.samp_nvalid, 2, L.valid_rank, cs, L.scan_tmp, stream);
+    if (rc) return rc;
+    k_valid_list<<<(cs + 255) / 256, 256, 0, stream>>>(R, cap, L.samp_off, L.samp_nvalid, L.valid_rank, L.valid_list, L.counters);
+    k_count_rays<<<(R + 255) / 256, 256, 0, stream>>>(R, L.ray_hit, L.counters);
+    PNB_CHECK_CUDA(cudaGetLastError());
+
+    *q = pnb_query_t{};
+    q->R = R; q->SR = SR; q->K = K; q->D = 0; q->cap_samples = cap;
+    q->nsamp = L.nsamp; q->samp_off = L.samp_off; q->steps = nullptr; q->samp_ray = L.samp_ray;
+    q->cand_pidx = const_cast<int32_t*>(d_sample_pidx); q->samp_nvalid = L.samp_nvalid; q->valid_list = L.valid_list;
+    q->valid_rank = L.valid_rank; q->ray_hit = L.ray_hit; q->counters = L.counters;
+    q->ray_rank = L.ray_rank; q->scan_tmp = L.scan_tmp;
+    q->xs_loc_w = d_sample_loc_w; q->xs_loc = d_sample_loc; q->xs_dir = d_sample_ray_dirs;
     return PNB_OK;
 }

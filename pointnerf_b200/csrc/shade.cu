@@ -157,8 +157,9 @@ __device__ __forceinline__ void dense8(const float* __restrict__ in, int sin_, f
 
 static_assert(offsetof(ShadeSmem, H) == sizeof(float) * TR * XS && TR * XS1 <= TR * (XS + HS), "F = 63 rows overlay X and H");
 
-// PP: per-point frames (pts.rw2c != NULL); F: point_features_dim (32 | 63); both compile-time parameters
-template <bool PP, int F>
+// PP: per-point frames (pts.rw2c != NULL); F: point_features_dim (32 | 63); XSAMP: explicit samples (the frustum query,
+// pair_inputs.cuh); all compile-time parameters
+template <bool PP, int F, bool XSAMP = false>
 __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     ShadeSmem& sm = *reinterpret_cast<ShadeSmem*>(smem_raw);
@@ -179,7 +180,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_shade_fwd(ShadeParams p) {
             const uint32_t s = have ? q.valid_list[vi] : 0xffffffffu;
             float* xr = &X1[row * XS_1];
             if (lane == 0) sm.samp[warp] = s;
-            const Fp32Pair pr = fp32_pair<PP>(q, p.pts, p.o, have, s, q.K, lane, &sm.view[warp][3]);
+            const Fp32Pair pr = fp32_pair<PP, XSAMP>(q, p.pts, p.o, have, s, q.K, lane, &sm.view[warp][3]);
             if (lane < 3) sm.view[warp][lane] = lane == 0 ? pr.ov.x : lane == 1 ? pr.ov.y : pr.ov.z;
             if (part == 0) sm.wc[row] = pr.wc;
             if (pr.g.valid) {
@@ -268,8 +269,12 @@ struct CompositeParams {
     float* opacity;
     float* bg_T;
     int8_t* ray_mask;
+    const float* bg_ray;   // BGR: [R,3]
 };
 
+// XSAMP: explicit samples (pair_inputs.cuh); BGR: per-ray background bg_ray instead of bg_color, added as the reference's fill_invalid
+// adds it (coarse_is_background * bg_ray, then + colour: each rounded, no contraction)
+template <bool XSAMP = false, bool BGR = false>
 __global__ void __launch_bounds__(128) k_composite(CompositeParams p) {
     int r = blockIdx.x * blockDim.x + threadIdx.x;
     const pnb_query_t& q = p.q;
@@ -279,18 +284,22 @@ __global__ void __launch_bounds__(128) k_composite(CompositeParams p) {
     if (p.ray_mask) p.ray_mask[r] = hit ? 1 : 0;
     float* op = p.opacity ? p.opacity + (size_t)r * SR : nullptr;
     if (!hit) {  // fill_invalid: background colour, zero opacity, is_background 1
-        p.ray_color[3 * r] = p.o.bg_color[0]; p.ray_color[3 * r + 1] = p.o.bg_color[1]; p.ray_color[3 * r + 2] = p.o.bg_color[2];
+        if (BGR) {
+            p.ray_color[3 * r] = p.bg_ray[3 * r]; p.ray_color[3 * r + 1] = p.bg_ray[3 * r + 1]; p.ray_color[3 * r + 2] = p.bg_ray[3 * r + 2];
+        } else {
+            p.ray_color[3 * r] = p.o.bg_color[0]; p.ray_color[3 * r + 1] = p.o.bg_color[1]; p.ray_color[3 * r + 2] = p.o.bg_color[2];
+        }
         if (p.bg_T) p.bg_T[r] = 1.0f;
         if (op) for (int j = 0; j < SR; ++j) op[j] = 0.f;
         return;
     }
     const int n = q.nsamp[r];
     const uint32_t s0 = q.samp_off[r];
-    const float3 dir = ray_dir(q, r);
-    float cm = slot_depth(q, p.o, r, n, 0, dir);  // cummax so far
+    const float3 dir = XSAMP ? make_float3(0.f, 0.f, 0.f) : ray_dir(q, r);
+    float cm = slot_depth<XSAMP>(q, p.o, r, n, 0, dir);  // cummax so far
     float T = 1.0f, cr = 0.f, cg = 0.f, cb = 0.f;
     for (int j = 0; j < SR; ++j) {
-        float rd = ray_dist_step(q, p.o, r, n, j, dir, cm);
+        float rd = ray_dist_step<XSAMP>(q, p.o, r, n, j, dir, cm);
         float sg = 0.f, rr = 0.f, gg = 0.f, bb = 0.f;
         bool valid = false;
         if (j < n && q.samp_nvalid[s0 + j] > 0) {
@@ -305,9 +314,15 @@ __global__ void __launch_bounds__(128) k_composite(CompositeParams p) {
         T = T * (1.0f - o1 + 1e-10f);
         if (op) op[j] = o1;
     }
-    p.ray_color[3 * r] = cr + p.o.bg_color[0] * T;
-    p.ray_color[3 * r + 1] = cg + p.o.bg_color[1] * T;
-    p.ray_color[3 * r + 2] = cb + p.o.bg_color[2] * T;
+    if (BGR) {
+        p.ray_color[3 * r] = __fadd_rn(__fmul_rn(T, p.bg_ray[3 * r]), cr);
+        p.ray_color[3 * r + 1] = __fadd_rn(__fmul_rn(T, p.bg_ray[3 * r + 1]), cg);
+        p.ray_color[3 * r + 2] = __fadd_rn(__fmul_rn(T, p.bg_ray[3 * r + 2]), cb);
+    } else {
+        p.ray_color[3 * r] = cr + p.o.bg_color[0] * T;
+        p.ray_color[3 * r + 1] = cg + p.o.bg_color[1] * T;
+        p.ray_color[3 * r + 2] = cb + p.o.bg_color[2] * T;
+    }
     if (p.bg_T) p.bg_T[r] = T;
 }
 
@@ -330,6 +345,7 @@ struct AuxParams {
     float* grad_conf;          // backward: [N], accumulated into
 };
 
+template <bool XSAMP = false>
 __global__ void __launch_bounds__(128) k_aux_outputs(AuxParams p) {
     const pnb_query_t& q = p.q;
     const int SR = q.SR, K = q.K;
@@ -341,8 +357,7 @@ __global__ void __launch_bounds__(128) k_aux_outputs(AuxParams p) {
     float3 l = make_float3(0.f, 0.f, 0.f);
     const int32_t* pid = nullptr;
     if (j < n) {
-        const float t = slot_t(q, r, j);
-        l = ray_pos(q, ray_dir(q, r), t);
+        l = slot_pos<XSAMP>(q, r, j);
         pid = q.cand_pidx + (size_t)(q.samp_off[r] + j) * K;
     }
     float w[PNB_MAX_K], wsum = 0.f;
@@ -419,7 +434,7 @@ struct ProbeParams {
     float* weight;             // [n_rows, K] or NULL (tests): w_k
 };
 
-template <int F>
+template <int F, bool XSAMP = false>
 __global__ void __launch_bounds__(128) k_probe_outputs(ProbeParams p) {
     const pnb_query_t& q = p.q;
     const int SR = q.SR, K = q.K, lane = threadIdx.x & 31;
@@ -458,7 +473,7 @@ __global__ void __launch_bounds__(128) k_probe_outputs(ProbeParams p) {
     float3 l = make_float3(0.f, 0.f, 0.f);
     const int32_t* pid = nullptr;
     if (oi < n) {
-        l = ray_pos(q, ray_dir(q, r), slot_t(q, r, oi));
+        l = slot_pos<XSAMP>(q, r, oi);
         pid = q.cand_pidx + (size_t)(q.samp_off[r] + oi) * K;
     }
     // the K weights and distances, every lane the same (K <= 8 points): k_aux_outputs' expressions in its k order
@@ -529,6 +544,8 @@ extern "C" int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, 
         PNB_REQUIRE(mlp->w[i] && mlp->b[i], PNB_ERR_INVALID, "pnb_shade_forward: MLP tensor %d is null", i);
     int F = 0;
     { const int rc = feat_check(pts, mlp, "pnb_shade_forward", &F); if (rc) return rc; }
+    const bool xs = q->xs_loc_w != nullptr;
+    { const int rc = xs_check(q, pts, F, "pnb_shade_forward"); if (rc) return rc; }
     static int smem_set[64] = {0}, n_sm_of[64] = {0};      // per device of this process
     int dev = 0;
     PNB_CHECK_CUDA(cudaGetDevice(&dev));
@@ -538,6 +555,7 @@ extern "C" int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, 
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true, PNB_FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false, PNB_FEAT_DTU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true, PNB_FEAT_DTU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false, PNB_FEAT_DTU, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
         PNB_CHECK_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
         smem_set[dev] = 1;
     }
@@ -546,7 +564,21 @@ extern "C" int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, 
     p.q = *q; p.pts = *pts; p.mlp = *mlp; p.o = *opts; p.sigma_rgb = (float4*)d_sigma_rgb;
     void (*kern)(ShadeParams) = F == PNB_FEAT ? (pts->rw2c ? k_shade_fwd<true, PNB_FEAT> : k_shade_fwd<false, PNB_FEAT>)
                                               : (pts->rw2c ? k_shade_fwd<true, PNB_FEAT_DTU> : k_shade_fwd<false, PNB_FEAT_DTU>);
+    if (xs) kern = k_shade_fwd<false, PNB_FEAT_DTU, true>;
     kern<<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
+    PNB_CHECK_CUDA(cudaGetLastError());
+    return PNB_OK;
+}
+
+static int composite(const pnb_query_t* q, const pnb_shade_opts_t* opts, const float* d_sigma_rgb, const float* d_bg_ray,
+                     float* d_ray_color, float* d_opacity, float* d_bg_T, int8_t* d_ray_mask, cudaStream_t stream) {
+    CompositeParams p;
+    p.q = *q; p.o = *opts; p.sigma_rgb = (const float4*)d_sigma_rgb;
+    p.ray_color = d_ray_color; p.opacity = d_opacity; p.bg_T = d_bg_T; p.ray_mask = d_ray_mask; p.bg_ray = d_bg_ray;
+    const bool xs = q->xs_loc_w != nullptr;
+    void (*kern)(CompositeParams) = d_bg_ray ? (xs ? k_composite<true, true> : k_composite<false, true>)
+                                             : (xs ? k_composite<true, false> : k_composite<false, false>);
+    kern<<<(q->R + 127) / 128, 128, 0, stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }
@@ -554,14 +586,15 @@ extern "C" int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, 
 extern "C" int pnb_composite_forward(const pnb_query_t* q, const pnb_shade_opts_t* opts, const float* d_sigma_rgb,
                                      float* d_ray_color, float* d_opacity, float* d_bg_T, int8_t* d_ray_mask,
                                      pnb_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
     PNB_REQUIRE(q && opts && d_sigma_rgb && d_ray_color, PNB_ERR_INVALID, "pnb_composite_forward: null argument");
-    CompositeParams p;
-    p.q = *q; p.o = *opts; p.sigma_rgb = (const float4*)d_sigma_rgb;
-    p.ray_color = d_ray_color; p.opacity = d_opacity; p.bg_T = d_bg_T; p.ray_mask = d_ray_mask;
-    k_composite<<<(q->R + 127) / 128, 128, 0, stream>>>(p);
-    PNB_CHECK_CUDA(cudaGetLastError());
-    return PNB_OK;
+    return composite(q, opts, d_sigma_rgb, nullptr, d_ray_color, d_opacity, d_bg_T, d_ray_mask, (cudaStream_t)stream_);
+}
+
+extern "C" int pnb_composite_forward_bg_ray(const pnb_query_t* q, const pnb_shade_opts_t* opts, const float* d_sigma_rgb,
+                                            const float* d_bg_ray, float* d_ray_color, float* d_opacity, float* d_bg_T,
+                                            int8_t* d_ray_mask, pnb_stream_t stream_) {
+    PNB_REQUIRE(q && opts && d_sigma_rgb && d_bg_ray && d_ray_color, PNB_ERR_INVALID, "pnb_composite_forward_bg_ray: null argument");
+    return composite(q, opts, d_sigma_rgb, d_bg_ray, d_ray_color, d_opacity, d_bg_T, d_ray_mask, (cudaStream_t)stream_);
 }
 
 extern "C" int pnb_aux_outputs(const pnb_query_t* q, const pnb_points_t* pts, const long long* d_rows, int n_rows, const float* d_opacity,
@@ -577,7 +610,8 @@ extern "C" int pnb_aux_outputs(const pnb_query_t* q, const pnb_points_t* pts, co
     p.q = *q; p.xyz = pts->xyz; p.conf = pts->conf; p.rows = d_rows; p.n_rows = n_rows; p.opacity = d_opacity;
     p.weight = d_weight; p.cc = d_conf_coefficient; p.blend = d_blend_weight; p.grad_cc = nullptr; p.grad_conf = nullptr;
     const long long n = (long long)n_rows * q->SR;
-    k_aux_outputs<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(p);
+    if (q->xs_loc_w) k_aux_outputs<true><<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(p);
+    else k_aux_outputs<false><<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }
@@ -599,7 +633,10 @@ extern "C" int pnb_probe_outputs(const pnb_query_t* q, const pnb_points_t* pts, 
     p.max_opacity = d_max_opacity; p.max_loc = d_max_loc; p.far_dist = d_far_dist; p.avg_color = d_avg_color; p.avg_dir = d_avg_dir;
     p.avg_conf = d_avg_conf; p.avg_emb = d_avg_emb; p.slot = d_slot; p.weight = d_weight;
     const unsigned blocks = (unsigned)((n_rows + 3) / 4);   // 4 rays (warps) per block
-    if (F == PNB_FEAT) k_probe_outputs<PNB_FEAT><<<blocks, 128, 0, stream>>>(p);
+    if (q->xs_loc_w) {
+        PNB_REQUIRE(F == PNB_FEAT_DTU, PNB_ERR_UNSUPPORTED, "pnb_probe_outputs: the frustum query's samples need point_features_dim 63");
+        k_probe_outputs<PNB_FEAT_DTU, true><<<blocks, 128, 0, stream>>>(p);
+    } else if (F == PNB_FEAT) k_probe_outputs<PNB_FEAT><<<blocks, 128, 0, stream>>>(p);
     else k_probe_outputs<PNB_FEAT_DTU><<<blocks, 128, 0, stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;

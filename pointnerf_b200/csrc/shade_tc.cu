@@ -114,12 +114,12 @@ __device__ __forceinline__ float seg_sum8(float v, int lane, int st, int cnt) {
 //   part 1 = operand columns 152..287 (PE of features 20..31, PE of the 6 distances), extras operand, weight*conf
 // FROZEN (part 1 only, one builder thread per row): the feature columns come from the per-point table, so the row is part 1
 // without the feature PE and with the distance PE at operand columns 0..63 (K blocks 0, 1); it also records the row's point.
-// PP: per-point frames (pair_inputs.cuh, point_frame).
+// PP: per-point frames (pair_inputs.cuh, point_frame).  XSAMP: explicit samples (the frustum query, pair_inputs.cuh).
 // F = 63 (not FROZEN; column order at tc::w1_row_f63), half HALF of the row:
 //   half 0: part 0 = PE of features 0..23; part 1 = PE of features 24..31, PE of the distances, extras, weight*conf, the row's point
 //   half 1: part 0 = raw features, PE of features 32..43; part 1 = PE of features 44..62 (the point is read back from sm.prow)
 // emb rows of 63 floats are not 16-byte aligned: scalar loads.
-template <int PART, bool FROZEN, bool PP, int F = PNB_FEAT, int HALF = 0, class SmemT>
+template <int PART, bool FROZEN, bool PP, int F = PNB_FEAT, int HALF = 0, bool XSAMP = false, class SmemT>
 __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& p, int row, int n_valid, int pvi, int pk, int pst, int pcnt) {
     using namespace tc;
     static_assert(PART == 0 || PART == 1, "two parts per row");
@@ -139,11 +139,12 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
     const pnb_query_t& q = p.q;
     int pidx = -1, p0 = 0;
     CandSample cs = {};
+    float3 lp = make_float3(0.f, 0.f, 0.f);
     if (W && HALF == 1) {
         pidx = sm.prow[row];
     } else if (pvi >= 0 && pvi < n_valid) {
         const uint32_t s = q.valid_list[pvi];
-        if (GEO) { cs = cand_sample(q, s); p0 = view_point<PP>(q, s); }
+        if (GEO) { cs = cand_sample<XSAMP>(q, s); p0 = view_point<PP>(q, s); if (XSAMP) lp = cand_pers<XSAMP>(q, s); }
         if (pk < q.K) pidx = q.cand_pidx[(size_t)s * q.K + pk];
     }
     if (FROZEN || (W && GEO)) sm.prow[row] = pidx;
@@ -153,7 +154,7 @@ __device__ __forceinline__ void build_pair_part(SmemT& sm, const ShadeTcParams& 
     float3 ov;
     if (GEO) {
         ov = view_in_points<PP>(p.pts, p.o, p0, cs.dir);
-        g = pair_geom<PP>(p.pts, p.o, pidx, cs.pos);
+        g = pair_geom<PP, XSAMP>(p.pts, p.o, pidx, cs.pos, lp);
         const float wsum = seg_sum8(g.w, row & 31, pst, pcnt);   // every lane takes part in the shuffles
         sm.wc[row] = valid ? norm_weight(g.w, wsum) * g.cc : 0.f;
     }
@@ -566,11 +567,12 @@ __device__ __forceinline__ uint32_t step_image(uint32_t j, bool frozen) {
 }  // namespace hw
 
 // O1: agg_intrp_order == 1 as a compile-time flag (the alpha dot product over the K-aggregated feature); PP: per-point frames
-// (pts.rw2c != NULL), compile-time as well, so that the uniform-frame builds keep their registers; F: point_features_dim (32 | 63).
+// (pts.rw2c != NULL), compile-time as well, so that the uniform-frame builds keep their registers; F: point_features_dim (32 | 63);
+// XSAMP: explicit samples (the frustum query, pair_inputs.cuh), instantiated for F = 63 with uniform frames.
 // F = 63, not FROZEN: layer 1 runs over 512 operand columns in two halves of 16 K steps; after the first half every wgmma that read it
 // retires (both warpgroups), the builders write the second half over it and the accumulator carries on.  FROZEN does not read the
 // features: only its layer-1 weight images differ.
-template <bool FROZEN, bool O1, bool PP, int F>
+template <bool FROZEN, bool O1, bool PP, int F, bool XSAMP = false>
 __global__ void __launch_bounds__(hw::NTHR_CTA, 1) k_shade_wg(ShadeTcParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -628,9 +630,9 @@ __global__ void __launch_bounds__(hw::NTHR_CTA, 1) k_shade_wg(ShadeTcParams p) {
                 const int cj = __shfl_sync(0xffffffffu, c, qr.j);
                 if (lane == 0 && part == 0) { sm.qhead[qw] = head; sm.qfirst[qw] = first; sm.qtotal[qw] = (uint32_t)total; }
                 const int pvi = qr.live ? (int)p.vorder[first + qr.j] : -1;
-                if (FROZEN) build_pair_part<1, true, PP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else if (part == 0) build_pair_part<0, false, PP, F>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
-                else build_pair_part<1, false, PP, F>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                if (FROZEN) build_pair_part<1, true, PP, PNB_FEAT, 0, XSAMP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else if (part == 0) build_pair_part<0, false, PP, F, 0, XSAMP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
+                else build_pair_part<1, false, PP, F, 0, XSAMP>(sm, p, row, n_valid, pvi, lane - qr.st, qr.st, qr.live ? cj : 1);
             }
             fence_proxy_async();
             named_bar_sync(1, hw::NTHR);
@@ -648,8 +650,8 @@ __global__ void __launch_bounds__(hw::NTHR_CTA, 1) k_shade_wg(ShadeTcParams p) {
                         pin<128>(acc);
                         named_bar_sync(1, hw::NTHR);
                         const int row = (warp & 3) * 32 + lane;
-                        if (warp < 4) build_pair_part<0, false, PP, F, 1>(sm, p, row, n_valid, -1, 0, 0, 1);
-                        else build_pair_part<1, false, PP, F, 1>(sm, p, row, n_valid, -1, 0, 0, 1);
+                        if (warp < 4) build_pair_part<0, false, PP, F, 1, XSAMP>(sm, p, row, n_valid, -1, 0, 0, 1);
+                        else build_pair_part<1, false, PP, F, 1, XSAMP>(sm, p, row, n_valid, -1, 0, 0, 1);
                         fence_proxy_async();
                         named_bar_sync(1, hw::NTHR);
                         wg::fence();
@@ -794,8 +796,8 @@ struct Smem {
 };
 }  // namespace hcw
 
-// PP: per-point frames (the view direction in the frame of each sample's slot-0 point)
-template <bool PP>
+// PP: per-point frames (the view direction in the frame of each sample's slot-0 point); XSAMP: explicit samples (pair_inputs.cuh)
+template <bool PP, bool XSAMP = false>
 __global__ void __launch_bounds__(hcw::NTHR_CTA, 1) k_color_wg(ColorTcParams p) {
     using namespace hcw;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -842,7 +844,7 @@ __global__ void __launch_bounds__(hcw::NTHR_CTA, 1) k_color_wg(ColorTcParams p) 
             for (int i = 0; i < 32; ++i) pe[i] = 0.f;
             if (vi < n_valid) {
                 const uint32_t s = q.valid_list[vi];
-                const float3 v = view_in_points<PP>(p.pts, p.o, view_point<PP>(q, s), ray_dir(q, cand_ray(q, s)));
+                const float3 v = view_in_points<PP>(p.pts, p.o, view_point<PP>(q, s), cand_view_dir<XSAMP>(q, s));
                 const float ov[3] = {v.x, v.y, v.z};
 #pragma unroll
                 for (int d = 0; d < 3; ++d) {     // ori=True layout: sin block (d*4+j) then cos block
@@ -1055,6 +1057,8 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
     PNB_REQUIRE(!frozen || d_point_pre, PNB_ERR_INVALID, "pnb_shade_forward_tc: PNB_TC_FROZEN needs the table of pnb_point_pre");
     int F = 0;
     { const int rc = feat_check(pts, mlp, "pnb_shade_forward_tc", &F); if (rc) return rc; }
+    const bool xs = q->xs_loc_w != nullptr;                  // explicit samples (the frustum query)
+    { const int rc = xs_check(q, pts, F, "pnb_shade_forward_tc"); if (rc) return rc; }
     static int configured[64] = {0}, n_sm_of[64] = {0};      // per device of this process (one process per GPU is the norm)
     int dev = 0;
     PNB_CHECK_CUDA(cudaGetDevice(&dev));
@@ -1065,7 +1069,7 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
     static_assert(sizeof(hw::Smem) + 128 <= kSmemMax, "pair kernel shared-memory carve-out exceeds the per-block limit");
     static_assert(sizeof(hcw::Smem) + 128 <= kSmemMax, "colour kernel shared-memory carve-out exceeds the per-block limit");
     if (!configured[dev]) {
-        const void* pair_kernels[16] = {
+        const void* pair_kernels[20] = {
             (const void*)k_shade_wg<false, false, false, PNB_FEAT>, (const void*)k_shade_wg<false, true, false, PNB_FEAT>,
             (const void*)k_shade_wg<true, false, false, PNB_FEAT>, (const void*)k_shade_wg<true, true, false, PNB_FEAT>,
             (const void*)k_shade_wg<false, false, true, PNB_FEAT>, (const void*)k_shade_wg<false, true, true, PNB_FEAT>,
@@ -1073,10 +1077,13 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
             (const void*)k_shade_wg<false, false, false, PNB_FEAT_DTU>, (const void*)k_shade_wg<false, true, false, PNB_FEAT_DTU>,
             (const void*)k_shade_wg<true, false, false, PNB_FEAT_DTU>, (const void*)k_shade_wg<true, true, false, PNB_FEAT_DTU>,
             (const void*)k_shade_wg<false, false, true, PNB_FEAT_DTU>, (const void*)k_shade_wg<false, true, true, PNB_FEAT_DTU>,
-            (const void*)k_shade_wg<true, false, true, PNB_FEAT_DTU>, (const void*)k_shade_wg<true, true, true, PNB_FEAT_DTU>};
+            (const void*)k_shade_wg<true, false, true, PNB_FEAT_DTU>, (const void*)k_shade_wg<true, true, true, PNB_FEAT_DTU>,
+            (const void*)k_shade_wg<false, false, false, PNB_FEAT_DTU, true>, (const void*)k_shade_wg<false, true, false, PNB_FEAT_DTU, true>,
+            (const void*)k_shade_wg<true, false, false, PNB_FEAT_DTU, true>, (const void*)k_shade_wg<true, true, false, PNB_FEAT_DTU, true>};
         for (const void* k : pair_kernels) PNB_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
         PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
         PNB_CHECK_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
         configured[dev] = 1;
     }
@@ -1107,6 +1114,9 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
                                           : (pp ? k_shade_wg<true, false, true, PNB_FEAT_DTU> : k_shade_wg<true, false, false, PNB_FEAT_DTU>))
                                     : (o1 ? (pp ? k_shade_wg<false, true, true, PNB_FEAT_DTU> : k_shade_wg<false, true, false, PNB_FEAT_DTU>)
                                           : (pp ? k_shade_wg<false, false, true, PNB_FEAT_DTU> : k_shade_wg<false, false, false, PNB_FEAT_DTU>)));
+        if (xs)
+            kern = frozen ? (o1 ? k_shade_wg<true, true, false, PNB_FEAT_DTU, true> : k_shade_wg<true, false, false, PNB_FEAT_DTU, true>)
+                          : (o1 ? k_shade_wg<false, true, false, PNB_FEAT_DTU, true> : k_shade_wg<false, false, false, PNB_FEAT_DTU, true>);
         kern<<<n_cta, hw::NTHR_CTA, smem_pair, stream>>>(p);
     }
     if (flags & PNB_TC_COLOR) {
@@ -1116,7 +1126,8 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
         ct.w3t = mlp->w[8]; ct.b3 = mlp->b[8];
         ct.hbar = w.hbar; ct.sigma = w.sigma; ct.hbar_cap = max_valid_samples; ct.sigma_rgb = (float4*)d_sigma_rgb; ct.err = d_err;
         ct.pts = *pts;
-        if (pts->rw2c) k_color_wg<true><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
+        if (xs) k_color_wg<false, true><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
+        else if (pts->rw2c) k_color_wg<true><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
         else k_color_wg<false><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
     }
     PNB_CHECK_CUDA(cudaGetLastError());

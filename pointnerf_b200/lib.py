@@ -34,7 +34,8 @@ class Query(C.Structure):
                 ("cand_pidx", C.c_void_p), ("samp_nvalid", C.c_void_p), ("valid_list", C.c_void_p),
                 ("valid_rank", C.c_void_p), ("ray_hit", C.c_void_p), ("ray_rank", C.c_void_p),
                 ("scan_tmp", C.c_void_p), ("counters", C.c_void_p), ("raydir", C.c_void_p), ("t", C.c_void_p),
-                ("t_ray_stride", C.c_int32), ("campos", C.c_float * 3)]
+                ("t_ray_stride", C.c_int32), ("campos", C.c_float * 3),
+                ("xs_loc_w", C.c_void_p), ("xs_loc", C.c_void_p), ("xs_dir", C.c_void_p)]
 
 
 class ShadeOpts(C.Structure):
@@ -70,7 +71,7 @@ SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes",
            "pnb_mlp_pack_bytes", "pnb_mlp_pack", "pnb_point_pre_bytes", "pnb_point_pre", "pnb_shade_tc_bytes", "pnb_shade_forward_tc",
            "pnb_shade_tc_tables", "pnb_shade_tc_buffers", "pnb_backward_bytes", "pnb_shade_backward", "pnb_backward_tables", "pnb_aux_outputs",
            "pnb_aux_conf_backward", "pnb_probe_outputs", "pnb_frustum_bytes", "pnb_frustum_build", "pnb_frustum_query_bytes", "pnb_frustum_query",
-           "pnb_frustum_export"]
+           "pnb_frustum_export", "pnb_frustum_samples_bytes", "pnb_frustum_samples", "pnb_composite_forward_bg_ray"]
 # test-only library (csrc/selftest/pnb200_selftest.h)
 SELFTEST_LIB_PATH = os.path.join(_HERE, "csrc", "libpnb200_selftest.so")
 SELFTEST_SYMBOLS = ["pnb_selftest_last_error", "pnb_umma_selftest", "pnb_umma_selftest2", "pnb_gemm_tc_test"]
@@ -123,6 +124,9 @@ def load():
     lib.pnb_composite_forward.restype = C.c_int
     lib.pnb_composite_forward.argtypes = [C.POINTER(Query), C.POINTER(ShadeOpts), C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.pnb_composite_forward_bg_ray.restype = C.c_int
+    lib.pnb_composite_forward_bg_ray.argtypes = [C.POINTER(Query), C.POINTER(ShadeOpts), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.pnb_aux_outputs.restype = C.c_int
     lib.pnb_aux_outputs.argtypes = [C.POINTER(Query), C.POINTER(Points), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p]
@@ -171,6 +175,11 @@ def load():
     lib.pnb_frustum_export.restype = C.c_int
     lib.pnb_frustum_export.argtypes = [C.POINTER(Frustum), C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_float,
                                        C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.pnb_frustum_samples_bytes.restype = C.c_size_t
+    lib.pnb_frustum_samples_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+    lib.pnb_frustum_samples.restype = C.c_int
+    lib.pnb_frustum_samples.argtypes = [C.POINTER(Query), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = lib
     return lib
 

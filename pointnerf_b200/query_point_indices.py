@@ -17,6 +17,9 @@ makes the reference's NeuralPoints use it unchanged (INTEGRATION.md).  Differenc
   * only NN 2, inverse 0, B 1, K <= 8 and SR <= 128 (the DTU scripts' configuration) are implemented: anything else raises;
   * no pycuda and no CPU path: the CUDA library must be present, otherwise lib.load() raises.
 The jitter (`uniform`, `gaussian`) and `pers2w` are the reference's own torch expressions, so they round the same way.
+
+`run_fused` is the entry point of the fused module (pointnerf_b200.ray_marching with wcoord_query 0): the same query and tuple, handed
+to the shading kernels in the sample-compacted layout of pnb_frustum_samples.  Its one host synchronisation is the one that sizes R'.
 """
 import numpy as np
 import torch
@@ -38,6 +41,39 @@ def hyperparameters(opt, h, w, intrinsic, near_depth, far_depth):
     scaled_vsize = (vsize * vscale).astype(np.float32)
     radius_limit, depth_limit = opt.radius_limit_scale * max(vsize[0], vsize[1]), opt.depth_limit_scale * vsize[2]
     return np.float32(radius_limit), np.float32(depth_limit), ranges, vsize, vdim, scaled_vsize, scaled_vdim, vscale
+
+
+def w2pers(point_xyz, camrotc2w, campos):
+    """NeuralPoints.w2pers (neural_points.py:604-610), the reference's expression: perspective coordinates (x/z, y/z, z) of [N,3] world
+    points for camera [1,3,3] / [1,3]."""
+    point_xyz_shift = point_xyz[None, ...] - campos[:, None, :]
+    xyz = torch.sum(camrotc2w[:, None, :, :] * point_xyz_shift[:, :, :, None], dim=-2)
+    xper = xyz[:, :, 0] / xyz[:, :, 2]
+    yper = xyz[:, :, 1] / xyz[:, :, 2]
+    return torch.stack([xper, yper, xyz[:, :, 2]], dim=-1)
+
+
+class FrustumSamples:
+    """One frustum query in the sample-compacted layout (pnb_query_t) the fused renderer reads: every slot of a hit ray is a
+    candidate sample, its geometry read in place from the querier's tuple, which this object keeps alive."""
+
+    def __init__(self, desc, ws, R, R2, SR, K, tup):
+        self.desc, self.ws, self.R, self.R2, self.SR, self.K = desc, ws, R, R2, SR, K
+        self.sample_pidx, self.sample_loc, self.sample_loc_w, self.sample_ray_dirs, self.ray_mask, self.vsize, self.ranges = tup
+        self._counters = None
+
+    def counters_tensor(self):
+        """The device int32[16] counters (PNB_QC_*) as a tensor view into the workspace."""
+        off = int(self.desc.counters) - self.ws.data_ptr()
+        return self.ws[off:off + 64].view(torch.int32)
+
+    @property
+    def counters(self):
+        """The counters on the host (PNB_QC_* names); the first access synchronises the stream."""
+        if self._counters is None:
+            h = self.counters_tensor().cpu()
+            self._counters = {k: int(h[i]) for k, i in _lib.QC.items()}
+        return self._counters
 
 
 class lighting_fast_querier():
@@ -170,6 +206,29 @@ class lighting_fast_querier():
             sample_loc_tensor = getattr(self, self.opt.shpnt_jitter, None)(sample_loc_tensor, vsize)
         sample_loc_w_tensor, sample_ray_dirs_tensor = self.pers2w(sample_loc_tensor, cam_rot_tensor, cam_pos_tensor)
         return sample_pidx_tensor, sample_loc_tensor, sample_loc_w_tensor, sample_ray_dirs_tensor, ray_mask[None], vsize, ranges
+
+    # ------------------------------------------------------------------ the fused module's entry point
+    def run_fused(self, xyz, campos, camrotc2w, pixel_idx, h, w, intrinsic, near, far):
+        """The query of forward() / render_full() with wcoord_query 0: the points' perspective coordinates (w2pers), query_points (one
+        host synchronisation for R'; the build is cached per view; jitter with opt.is_train, drawn as the reference draws it), then
+        pnb_frustum_samples.  xyz [N,3]; campos [1,3] and camrotc2w [1,3,3] device tensors; pixel_idx [.., 2]; h, w, intrinsic [3,3],
+        near, far as NeuralPoints.forward passes them to the querier.  Returns a FrustumSamples."""
+        lib = _lib.load()
+        dev = xyz.device
+        pers = w2pers(xyz, camrotc2w, campos)
+        pix = pixel_idx.reshape(1, -1, 2).to(torch.int32)
+        tup = self.query_points(pix, pers, xyz[None], torch.tensor([xyz.shape[0]], dtype=torch.int32), h, w, intrinsic, near, far,
+                                None, campos, camrotc2w)
+        pidx, loc, loc_w, dirs, mask = (t[0].contiguous() for t in tup[:5])
+        R, R2 = pix.shape[1], int(pidx.shape[0])
+        SR, K = int(self.opt.SR), int(self.opt.K)
+        nb = lib.pnb_frustum_samples_bytes(R, R2, SR)
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)    # per call: a training step's backward still reads the previous one
+        desc = _lib.Query()
+        _lib.check(lib.pnb_frustum_samples(_lib.C.byref(desc), ws.data_ptr(), ws.numel(), mask.data_ptr(), R, R2, SR, K,
+                                           pidx.data_ptr(), loc_w.data_ptr(), loc.data_ptr(), dirs.data_ptr(),
+                                           torch.cuda.current_stream(dev).cuda_stream), "pnb_frustum_samples")
+        return FrustumSamples(desc, ws, R, R2, SR, K, (pidx, loc, loc_w, dirs, mask, tup[5], tup[6]))
 
     # ------------------------------------------------------------------ query_point_indices.py:102-126 (the reference's expressions)
     def pers2w(self, point_xyz_pers, camrotc2w, campos):

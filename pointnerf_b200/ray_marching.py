@@ -17,10 +17,12 @@ import math
 import os
 import weakref
 
+import numpy as np
 import torch
 import torch.nn as nn
 
 from . import lib as _lib
+from . import query_point_indices as _frustum
 from .point_query import lighting_fast_querier, make_cam_opts
 
 MLP_KEYS = ("block1.0", "block1.2", "block3.0", "block3.2", "alpha_branch.0",
@@ -63,6 +65,16 @@ _DEFAULTS = dict(view_ori=0, act_super=1, agg_weight_norm=1, apply_pnt_mask=1, w
                  shading_feature_mlp_layer2=0)
 
 
+# the options every shipped wcoord_query 0 script has, as check_opt compares them (str of the value)
+_FRUSTUM_REQUIRED = dict(point_features_dim="63", point_conf_mode="01", point_dir_mode="01", point_color_mode="01", NN="2",
+                         raydist_mode_unit="1")
+
+
+def is_frustum(opt):
+    """True when the module shades the perspective-frustum query's samples (wcoord_query 0)."""
+    return int(getattr(opt, "wcoord_query", -1)) == 0
+
+
 def check_opt(opt):
     """Reject (loudly) every option value outside the implemented configuration (SURVEY 8b)."""
     for k, want in _REQUIRED.items():
@@ -93,9 +105,13 @@ def check_opt(opt):
     if getattr(opt, "prob", 0) not in (0, 1):
         raise NotImplementedError("pnb200: opt.prob must be 0 or 1")
     if int(getattr(opt, "wcoord_query", -1)) == 0:
-        # the perspective-frustum query has its own drop-in (pointnerf_b200.query_point_indices); the fused module only runs the world grid
-        raise NotImplementedError("pnb200: wcoord_query=0 (perspective-frustum query) is not part of the fused module; "
-                                  "use pointnerf_b200.query_point_indices as the reference's querier")
+        # the perspective-frustum query (pointnerf_b200.query_point_indices) is shaded in the configuration of every shipped script that
+        # uses it (the DTU scripts): F = 63, point modes 01, NN 2, raydist_mode_unit 1; per-point frames are refused at run time
+        bad = ["%s=%r" % (k, getattr(opt, k, None)) for k, want in _FRUSTUM_REQUIRED.items() if str(getattr(opt, k, None)) != want]
+        if bad:
+            raise NotImplementedError("pnb200: wcoord_query=0 (perspective-frustum query) is implemented for the DTU scripts' "
+                                      "configuration only (%s); this opt has %s"
+                                      % (", ".join("%s %s" % kv for kv in _FRUSTUM_REQUIRED.items()), ", ".join(bad)))
     if float(getattr(opt, "xyz_grad", 0) or 0) > 0:
         # the fused backward produces no d/d(xyz) (every shipped script has xyz_grad = 0): refuse instead of silently freezing xyz
         raise NotImplementedError("pnb200: xyz_grad > 0 (point positions as trainable parameters) is outside the implemented hot path")
@@ -249,7 +265,8 @@ class NeuralPoints(nn.Module):
         self.xyz = None
         self.points_embeding = self.points_conf = self.points_dir = self.points_color = None
         self.Rw2c = torch.eye(3)
-        self.querier = lighting_fast_querier(device, opt)
+        # wcoord_query 0: the perspective-frustum querier (the reference's default query), otherwise the world grid
+        self.querier = _frustum.lighting_fast_querier(device, opt) if is_frustum(opt) else lighting_fast_querier(device, opt)
 
     def set_points(self, points_xyz, points_embeding, points_color=None, points_dir=None, points_conf=None,
                    parameter=True, Rw2c=None, as_stored=False, **_):
@@ -374,8 +391,6 @@ class _RenderFn(torch.autograd.Function):
         ctx.q = q
         ctx.generation = mod._generation          # the backward recomputes from the query / sigma_rgb buffers of THIS run
         ctx.o = mod._last_opts
-        ctx.n_valid = q.counters["n_valid"]
-        ctx.n_pairs = q.counters["n_pairs"]
         ctx.sigma_rgb = mod._sigma_rgb          # forward (sigma, rgb) per candidate; valid until the next _run
         ctx.needs = [t.requires_grad for t in (emb, color, pdir, conf)]
         ctx.mlp_shapes = [tuple(t.shape) for t in mlp_params]
@@ -397,6 +412,7 @@ class _RenderFn(torch.autograd.Function):
                                 "before the next forward")
         npnts = mod.neural_points
         dev = ctx.sigma_rgb.device
+        n_valid, n_pairs = q.counters["n_valid"], q.counters["n_pairs"]     # the frustum query reads them here (one synchronisation)
         g_color = _upstream_grad(g_color, ctx.shapes[0], "coarse_raycolor")
         g_op = _upstream_grad(g_op, ctx.shapes[1], "coarse_point_opacity")
         g_bg = _upstream_grad(g_bg, ctx.shapes[2], "coarse_is_background")
@@ -407,7 +423,7 @@ class _RenderFn(torch.autograd.Function):
             outs.append(torch.zeros(shape, dtype=torch.float32, device=dev) if need else None)
         dwt = [torch.zeros_like(w) for w in mod._mlp.wt]
         dbs = [torch.zeros_like(b) for b in mod._mlp.bias]
-        nb = lib.pnb_backward_bytes(max(ctx.n_valid, 1), q.desc.cap_samples, F)
+        nb = lib.pnb_backward_bytes(max(n_valid, 1), q.desc.cap_samples, F)
         if getattr(mod, "_bwd_ws", None) is None or mod._bwd_ws.numel() < nb:
             mod._bwd_ws = torch.empty(nb, dtype=torch.uint8, device=dev)
         wp = (_lib.C.c_void_p * 9)(*[t.data_ptr() for t in dwt])
@@ -422,8 +438,8 @@ class _RenderFn(torch.autograd.Function):
         # (fp32-faithful LeakyReLU masks) | 2 (diagnostic) three-part split in every tensor-core GEMM
         flags = int(getattr(mod.opt, "pnb_bwd_fp32", 0))
         _lib.check(lib.pnb_shade_backward(_lib.C.byref(q.desc), _lib.C.byref(pts), _lib.C.byref(mlp), _lib.C.byref(ctx.o),
-                                          ctx.sigma_rgb.data_ptr(), ptr(g_color), ptr(g_op), ptr(g_bg), int(ctx.n_valid),
-                                          int(ctx.n_pairs), ptr(outs[0]),
+                                          ctx.sigma_rgb.data_ptr(), ptr(g_color), ptr(g_op), ptr(g_bg), int(n_valid),
+                                          int(n_pairs), ptr(outs[0]),
                                           ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), wp, bp, mod._bwd_ws.data_ptr(),
                                           mod._bwd_ws.numel(), flags, mod._bwd_err.data_ptr(), stream), "pnb_shade_backward")
         grads = []
@@ -535,7 +551,7 @@ def _init_state(mod):
     mod._pnb_ready = True
 
 
-_PATCHED = ("forward", "_run", "check_errors", "render_full", "_point_pre", "_poll_status", "_queue_status")
+_PATCHED = ("forward", "_run", "check_errors", "render_full", "_point_pre", "_poll_status", "_queue_status", "_frustum_query")
 
 
 def install_into(reference_cls):
@@ -604,7 +620,9 @@ class NeuralPointsRayMarching(nn.Module):
                 raise _lib.PnbError("pnb200: tensor-core pipeline time-out (code %d) in an earlier render_full()" % err)
 
     # -------------------------------------------------------------------------------------------------
-    def _run(self, campos, raydir, camrotc2w, near, far, bg_color, want_counters, t=None, frozen=False):
+    def _run(self, campos, raydir, camrotc2w, near, far, bg_color, want_counters, t=None, frozen=False, view=None, bg_ray=None):
+        """view (wcoord_query 0): dict(pixel_idx, h, w, intrinsic) of the frustum query.  bg_ray [R,3]: the per-ray background of
+        render_full (pnb_composite_forward_bg_ray) instead of bg_color."""
         if not getattr(self, "_pnb_ready", False):
             _init_state(self)           # reference module patched by install_into(): state is created lazily
         lib = _lib.load()
@@ -615,12 +633,17 @@ class NeuralPointsRayMarching(nn.Module):
         # camera scalars go to the kernels by value: host lists / CPU tensors cost nothing, device tensors
         # cost one small D2H copy (the reference does the same with near/far/intrinsic, neural_points.py:704)
         cp, rt, bg = _to_list(campos)[:3], _to_list(camrotc2w)[:9], _to_list(bg_color)[:3]
-        q = npnts.querier.run_query(npnts.xyz.detach(), raydir, cp, float(near), float(far), t=t, want_counters=want_counters)
+        frustum = is_frustum(opt)
+        if frustum:
+            q, vsize_z = self._frustum_query(campos, camrotc2w, near, far, view, dev)
+        else:
+            q = npnts.querier.run_query(npnts.xyz.detach(), raydir, cp, float(near), float(far), t=t, want_counters=want_counters)
+            vsize_z = float(opt.vsize[2])
         # per-point frames go to the kernels through pnb_points_t.rw2c (read in place); the uniform slot of the options is unused then
         o = make_cam_opts(cp, rt, Rw2c=None if per_point_rw2c(npnts) else rw2c_host_of(npnts),
-                          vsize_z=float(opt.vsize[2]), bg_color=bg, raydist_mode_unit=int(getattr(opt, "raydist_mode_unit", 0)),
+                          vsize_z=vsize_z, bg_color=bg, raydist_mode_unit=int(getattr(opt, "raydist_mode_unit", 0)),
                           agg_intrp_order=int(getattr(opt, "agg_intrp_order", 2)))
-        cap = q.desc.cap_samples
+        cap = max(q.desc.cap_samples, 1)        # a frustum query without a hit ray lists no candidate
         self._generation += 1
         if self._sigma_rgb is None or self._sigma_rgb.shape[0] < cap or self._sigma_rgb.device != dev:
             self._sigma_rgb = torch.empty((cap, 4), dtype=torch.float32, device=dev)
@@ -637,7 +660,11 @@ class NeuralPointsRayMarching(nn.Module):
             # the next call (_poll_status)
             per_ray = max(float(getattr(opt, "pnb_max_valid_per_ray", 10)), 1.25 * self._valid_per_ray)
             max_valid = int(min(q.R * q.SR, max(min(1 << 20, q.R * q.SR), math.ceil(q.R * per_ray))))
-            if want_counters and getattr(q, "counters", None):
+            if frustum:
+                # every valid sample is a listed slot of a hit ray: R' SR bounds the count without reading it (forward() pays for
+                # that bound; a whole frame keeps the estimate, checked as for the world query)
+                max_valid = min(max_valid, q.R2 * q.SR) if not want_counters else q.R2 * q.SR
+            elif want_counters and getattr(q, "counters", None):
                 n_valid = int(q.counters.get("n_valid", 0))
                 self._valid_per_ray = max(self._valid_per_ray, n_valid / max(q.R, 1))
                 max_valid = max(max_valid, n_valid)
@@ -665,12 +692,40 @@ class NeuralPointsRayMarching(nn.Module):
         opacity = torch.empty((R, SR), dtype=torch.float32, device=dev)
         bg_T = torch.empty((R,), dtype=torch.float32, device=dev)
         ray_mask = torch.empty((R,), dtype=torch.int8, device=dev)
-        _lib.check(lib.pnb_composite_forward(_lib.C.byref(q.desc), _lib.C.byref(o), self._sigma_rgb.data_ptr(),
-                                             ray_color.data_ptr(), opacity.data_ptr(), bg_T.data_ptr(),
-                                             ray_mask.data_ptr(), stream), "pnb_composite_forward")
+        if bg_ray is not None:
+            bg_ray = bg_ray.reshape(R, 3).to(dev, torch.float32).contiguous()
+            _lib.check(lib.pnb_composite_forward_bg_ray(_lib.C.byref(q.desc), _lib.C.byref(o), self._sigma_rgb.data_ptr(), bg_ray.data_ptr(),
+                                                        ray_color.data_ptr(), opacity.data_ptr(), bg_T.data_ptr(),
+                                                        ray_mask.data_ptr(), stream), "pnb_composite_forward_bg_ray")
+        else:
+            _lib.check(lib.pnb_composite_forward(_lib.C.byref(q.desc), _lib.C.byref(o), self._sigma_rgb.data_ptr(),
+                                                 ray_color.data_ptr(), opacity.data_ptr(), bg_T.data_ptr(),
+                                                 ray_mask.data_ptr(), stream), "pnb_composite_forward")
         self.last = q
         self._last_opts = o
         return q, ray_color, opacity, bg_T, ray_mask
+
+    def _frustum_query(self, campos, camrotc2w, near, far, view, dev):
+        """The perspective-frustum query of one call (wcoord_query 0) and the ray-distance voxel depth of its grid (vsize[2] of the
+        frustum grid, neural_points_volumetric_model.py:272).  view: dict(pixel_idx, h, w, intrinsic), as forward() receives them."""
+        npnts = self.neural_points
+        if view is None or any(view.get(k) is None for k in ("pixel_idx", "h", "w", "intrinsic")):
+            raise ValueError("pnb200: wcoord_query=0 needs pixel_idx, h, w and intrinsic (the frustum query's view)")
+        if per_point_rw2c(npnts):
+            raise NotImplementedError("pnb200: wcoord_query=0 with per-point frames (Rw2c [N,3,3]) is outside the implemented hot path")
+        if not hasattr(npnts.querier, "run_fused"):
+            raise NotImplementedError("pnb200: wcoord_query=0 needs pointnerf_b200.query_point_indices.lighting_fast_querier as the querier")
+        # as NeuralPoints.forward hands them over (neural_points.py:704): intrinsic[0] in its own dtype, h and w as numpy integers
+        intr = view["intrinsic"]
+        intr = np.asarray(intr.detach().cpu().numpy() if isinstance(intr, torch.Tensor) else intr)
+        intr = intr[0] if intr.ndim == 3 else intr
+        h, w = (int(torch.max(torch.as_tensor(v))) for v in (view["h"], view["w"]))
+        cp = torch.as_tensor(campos, dtype=torch.float32).to(dev).reshape(1, 3)
+        rot = torch.as_tensor(camrotc2w, dtype=torch.float32).to(dev).reshape(1, 3, 3)
+        pix = torch.as_tensor(view["pixel_idx"]).to(dev)
+        # near / far as NeuralPoints.forward hands them to the querier (float32 numpy scalars, neural_points.py:704)
+        q = npnts.querier.run_fused(npnts.xyz.detach(), cp, rot, pix, np.int64(h), np.int64(w), intr, np.float32(near), np.float32(far))
+        return q, float(q.vsize[2])
 
     def check_errors(self):
         """Synchronising check of the device-side status of the tensor-core path: raises PnbOverflow (after enlarging the
@@ -713,14 +768,18 @@ class NeuralPointsRayMarching(nn.Module):
         ev.record(torch.cuda.current_stream(dev))
         self._status_pending.append((ev, host, q.R))
 
-    def render_full(self, campos, raydir, camrotc2w, near, far, bg_color, t=None, probe=False):
+    def render_full(self, campos, raydir, camrotc2w, near, far, bg_color, t=None, probe=False, bg_ray=None, view=None):
         """Full-R outputs, fill_invalid semantics, no host sync: dict(coarse_raycolor [1,R,3],
         coarse_point_opacity [1,R,SR], coarse_is_background [1,R,1], ray_mask [1,R]).  No gradients (frozen-cloud pipeline).
         probe=True: also the seven probe outputs of point growing (probe_keys, [1,R,C]; zeros where a ray missed, as the reference's
         unmask fills them), one more kernel on the same query.
+        bg_ray [1,R,3] (bgmodel plane): the model shell's fill_invalid in the kernel, bg_T * bg_ray + colour for a hit ray and bg_ray for
+        a miss (bg_color is not used).  view (wcoord_query 0): dict(pixel_idx, h, w, intrinsic) of the frustum query, whose one host
+        synchronisation (for R') is the only one of the call.
         The device status of the call (workspace overflow, time-out) is copied to pinned memory behind the kernels and raised
         by a LATER call or by check_errors(); runner.render_image / probe_image check it before returning."""
-        q, ray_color, opacity, bg_T, ray_mask = self._run(campos, raydir, camrotc2w, near, far, bg_color, False, t=t, frozen=True)
+        q, ray_color, opacity, bg_T, ray_mask = self._run(campos, raydir, camrotc2w, near, far, bg_color, False, t=t, frozen=True,
+                                                          view=view, bg_ray=bg_ray)
         out = dict(coarse_raycolor=ray_color[None], coarse_point_opacity=opacity[None],
                    coarse_is_background=bg_T[None, :, None], ray_mask=ray_mask[None])
         if probe:
@@ -731,11 +790,15 @@ class NeuralPointsRayMarching(nn.Module):
     def forward(self, campos, raydir, gt_image=None, bg_color=None, camrotc2w=None, pixel_idx=None, near=None,
                 far=None, focal=None, h=None, w=None, intrinsic=None, **kargs):
         if "bg_ray" in kargs:
-            raise NotImplementedError("pnb200: bg_ray input is not part of the implemented hot path")
+            # bgmodel plane: the reference composites without a background (bg_color = None, neural_points_volumetric_model.py:294-295)
+            # and the model shell's fill_invalid adds coarse_is_background * bg_ray
+            bg_color = None
         near_f = float(torch.min(near)) if isinstance(near, torch.Tensor) else float(near)
         far_f = float(torch.max(far)) if isinstance(far, torch.Tensor) else float(far)
         bg = bg_color if bg_color is not None else torch.zeros(3)
-        run_args = (campos, raydir, camrotc2w, near_f, far_f, bg, True)
+        frustum = is_frustum(self.opt)
+        view = dict(pixel_idx=pixel_idx, h=h, w=w, intrinsic=intrinsic) if frustum else None
+        run_args = (campos, raydir, camrotc2w, near_f, far_f, bg, True, None, False, view)
         npnts, agg = self.neural_points, self.aggregator
         train = torch.is_grad_enabled() and any(
             t is not None and t.requires_grad for t in
@@ -749,19 +812,24 @@ class NeuralPointsRayMarching(nn.Module):
                                                                  npnts.points_dir, npnts.points_conf, *mlp_params)
             q = self.last
         else:
-            q, ray_color, opacity, bg_T, ray_mask = self._run(*run_args, frozen=True)
+            q, ray_color, opacity, bg_T, ray_mask = self._run(*run_args[:8], frozen=True, view=view)
         # the shading workspace was sized from the query counters (no overflow possible); a pipeline time-out of this call or of the
         # previous backward is raised by the next call / check_errors() instead of stalling the host here until the forward has finished
         self._queue_status(q, ray_color.device)
         # compact to the R' rays the reference returns (one host sync already paid for the counters)
         # (the number of hit rays is already on the host with the query counters: no second synchronisation for the compaction)
-        inds = torch.nonzero_static(ray_mask, size=int(q.counters["R2"]))[:, 0] if getattr(q, "counters", None) else torch.nonzero(ray_mask)[:, 0]
+        n_hit = q.R2 if frustum else (int(q.counters["R2"]) if getattr(q, "counters", None) else None)
+        inds = torch.nonzero_static(ray_mask, size=n_hit)[:, 0] if n_hit is not None else torch.nonzero(ray_mask)[:, 0]
         out = {}
         out["coarse_raycolor"] = ray_color[inds][None]
         out["coarse_point_opacity"] = opacity[inds][None]
         out["coarse_is_background"] = bg_T[inds][None, :, None]
-        # queried_shading: 1 where no sample of the ray is valid (:290) -- rays in R' always have one
-        out["queried_shading"] = torch.zeros((1, inds.shape[0], 3), dtype=torch.float32, device=ray_color.device)
+        # queried_shading: 1 where no sample of the ray is valid (:290) -- rays in R' of the world query always have one; a hit ray of
+        # the frustum query (its pixel's column is occupied) may have none
+        if frustum:
+            out["queried_shading"] = (~(q.sample_pidx >= 0).any(-1).any(-1))[None, :, None].repeat(1, 1, 3).to(torch.float32)
+        else:
+            out["queried_shading"] = torch.zeros((1, inds.shape[0], 3), dtype=torch.float32, device=ray_color.device)
         out["ray_mask"] = ray_mask[None]
         opt = self.opt
         want_aux = (getattr(opt, "sparse_loss_weight", 0) > 0) or ("conf_coefficient" in getattr(opt, "zero_one_loss_items", [])) \
