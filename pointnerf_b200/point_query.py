@@ -128,6 +128,24 @@ def make_cam_opts(campos, camrotc2w, Rw2c=None, vsize_z=0.0, bg_color=(1., 1., 1
     return o
 
 
+def grid_hyperparameters(point_xyz_w_tensor, vsize_np, scaled_vsize_np, vscale_np, kernel_size, ranges):
+    """The world grid of point_query.py:47-71 (and query_point_indices_worldcoords.py:46-77, the same expressions): the points' box,
+    clipped to `ranges` and padded by half a kernel of scaled voxels.  Returns ranges_tensor ([6] on the points' device), scaled_vdim_np
+    (int32 [3]) and vdim_np (float64 [3], before the division by vscale)."""
+    min_xyz, max_xyz = torch.min(point_xyz_w_tensor, dim=-2)[0][0], torch.max(point_xyz_w_tensor, dim=-2)[0][0]
+    if ranges is not None:
+        ranges_min = torch.as_tensor(ranges[:3], dtype=torch.float32, device=min_xyz.device)
+        ranges_max = torch.as_tensor(ranges[3:], dtype=torch.float32, device=min_xyz.device)
+        min_xyz, max_xyz = torch.maximum(min_xyz, ranges_min), torch.minimum(max_xyz, ranges_max)
+    pad = torch.as_tensor(scaled_vsize_np * np.asarray(kernel_size) / 2, device=min_xyz.device, dtype=torch.float32)
+    min_xyz = min_xyz - pad
+    max_xyz = max_xyz + pad
+    ranges_tensor = torch.cat([min_xyz, max_xyz], dim=-1)
+    vdim_np = (max_xyz - min_xyz).cpu().numpy() / np.asarray(vsize_np, dtype=np.float64)
+    scaled_vdim_np = np.ceil(vdim_np / vscale_np).astype(np.int32)
+    return ranges_tensor, scaled_vdim_np, vdim_np
+
+
 class lighting_fast_querier():
     """Drop-in for point_query.py:25-108 (same name on purpose)."""
 
@@ -141,29 +159,33 @@ class lighting_fast_querier():
             raise NotImplementedError("pnb200: --inverse > 0 (disparity-linear ray generation) is outside the "
                                       "implemented hot path")
         self.count = 0
-        # cached at construction exactly like the reference (point_query.py:35-42)
-        self.radius_limit_np = np.asarray(self.opt.radius_limit_scale * max(self.opt.vsize[0], self.opt.vsize[1])).astype(np.float32)
-        self.vscale_np = np.array(self.opt.vscale, dtype=np.int32)
-        self.scaled_vsize_np = (np.asarray(self.opt.vsize, dtype=np.float64) * self.vscale_np).astype(np.float32)
+        self._read_options()
         self.scaled_vsize_tensor = torch.as_tensor(self.scaled_vsize_np, device=self.device)
-        self.kernel_size = np.asarray(self.opt.kernel_size, dtype=np.int32)
         self.kernel_size_tensor = torch.as_tensor(self.kernel_size, device=self.device)
-        self.query_size = np.asarray(self.opt.query_size, dtype=np.int32)
         self.query_size_tensor = torch.as_tensor(self.query_size, device=self.device)
-        if self.opt.K > _lib.MAX_K:
-            raise NotImplementedError("pnb200: K=%d > 8; the reference kernel's neighbour buffer is KN=8 "
-                                      "(query_worldcoords.cu:14), larger K is undefined there" % self.opt.K)
-        if self.opt.SR > _lib.MAX_SR:
-            raise NotImplementedError("pnb200: SR=%d > %d" % (self.opt.SR, _lib.MAX_SR))
         self.parity_slot0 = bool(getattr(self.opt, "pnb_parity_slot0", 1))
         self._grid = None
         self._grid_key = None
         self._hyper = None
         self._ws = None
         self._t_cache = {}
+        self.n_builds = 0
         self.last_grid_counters = None
         self.last_query_counters = None
         self.last_query = None
+
+    def _read_options(self):
+        """The query options, read here once at construction exactly like the reference (point_query.py:35-42)."""
+        if self.opt.K > _lib.MAX_K:
+            raise NotImplementedError("pnb200: K=%d > 8; the reference kernel's neighbour buffer is KN=8 "
+                                      "(query_worldcoords.cu:14), larger K is undefined there" % self.opt.K)
+        if self.opt.SR > _lib.MAX_SR:
+            raise NotImplementedError("pnb200: SR=%d > %d" % (self.opt.SR, _lib.MAX_SR))
+        self.radius_limit_np = np.asarray(self.opt.radius_limit_scale * max(self.opt.vsize[0], self.opt.vsize[1])).astype(np.float32)
+        self.vscale_np = np.array(self.opt.vscale, dtype=np.int32)
+        self.scaled_vsize_np = (np.asarray(self.opt.vsize, dtype=np.float64) * self.vscale_np).astype(np.float32)
+        self.kernel_size = np.asarray(self.opt.kernel_size, dtype=np.int32)
+        self.query_size = np.asarray(self.opt.query_size, dtype=np.int32)
 
     def clean_up(self):
         self._grid = None
@@ -174,29 +196,23 @@ class lighting_fast_querier():
 
     # ------------------------------------------------------------------ point_query.py:47-71
     def get_hyperparameters(self, vsize_np, point_xyz_w_tensor, ranges=None):
-        min_xyz, max_xyz = torch.min(point_xyz_w_tensor, dim=-2)[0][0], torch.max(point_xyz_w_tensor, dim=-2)[0][0]
-        if ranges is not None:
-            ranges_min = torch.as_tensor(ranges[:3], dtype=torch.float32, device=min_xyz.device)
-            ranges_max = torch.as_tensor(ranges[3:], dtype=torch.float32, device=min_xyz.device)
-            min_xyz, max_xyz = torch.maximum(min_xyz, ranges_min), torch.minimum(max_xyz, ranges_max)
-        pad = torch.as_tensor(self.scaled_vsize_np * np.asarray(self.opt.kernel_size) / 2, device=min_xyz.device, dtype=torch.float32)
-        min_xyz = min_xyz - pad
-        max_xyz = max_xyz + pad
-        ranges_tensor = torch.cat([min_xyz, max_xyz], dim=-1)
-        vdim_np = (max_xyz - min_xyz).cpu().numpy() / np.asarray(vsize_np, dtype=np.float64)
-        scaled_vdim_np = np.ceil(vdim_np / self.vscale_np).astype(np.int32)
+        ranges_tensor, scaled_vdim_np, _ = grid_hyperparameters(point_xyz_w_tensor, vsize_np, self.scaled_vsize_np, self.vscale_np,
+                                                                self.opt.kernel_size, ranges)
         return ranges_tensor, vsize_np, scaled_vdim_np
 
     def _grid_for(self, xyz):
         """xyz: [N,3] contiguous fp32 on the device.  Rebuilt only when the point cloud changed."""
         key = (xyz.data_ptr(), xyz._version, xyz.shape[0], tuple(float(v) for v in self.opt.ranges) if self.opt.ranges is not None else None)
         if self._grid is None or key != self._grid_key:
-            ranges_tensor, vsize_np, scaled_vdim_np = self.get_hyperparameters(self.opt.vsize, xyz[None], ranges=self.opt.ranges)
+            vsize_np = self.opt.vsize
+            ranges_tensor, scaled_vdim_np, _ = grid_hyperparameters(xyz[None], vsize_np, self.scaled_vsize_np, self.vscale_np,
+                                                                    self.opt.kernel_size, self.opt.ranges)
             ranges_np = ranges_tensor.cpu().numpy()
             max_o = self.opt.max_o if self.opt.max_o is not None else xyz.shape[0]
             self._grid = VoxelGrid(xyz, ranges_np[:3], self.scaled_vsize_np, scaled_vdim_np, self.query_size, max_o,
                                    self.opt.P, parity_slot0=self.parity_slot0)
             self._grid_key = key
+            self.n_builds += 1
             self._hyper = (ranges_tensor, ranges_np, vsize_np, scaled_vdim_np)
             self.last_grid_counters = self._grid.counters
         return self._grid

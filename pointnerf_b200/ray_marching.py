@@ -23,6 +23,7 @@ import torch.nn as nn
 
 from . import lib as _lib
 from . import query_point_indices as _frustum
+from . import query_point_indices_worldcoords as _worldcoords
 from .point_query import lighting_fast_querier, make_cam_opts
 
 MLP_KEYS = ("block1.0", "block1.2", "block3.0", "block3.2", "alpha_branch.0",
@@ -265,8 +266,14 @@ class NeuralPoints(nn.Module):
         self.xyz = None
         self.points_embeding = self.points_conf = self.points_dir = self.points_color = None
         self.Rw2c = torch.eye(3)
-        # wcoord_query 0: the perspective-frustum querier (the reference's default query), otherwise the world grid
-        self.querier = _frustum.lighting_fast_querier(device, opt) if is_frustum(opt) else lighting_fast_querier(device, opt)
+        # wcoord_query 0: the perspective-frustum querier (the reference's default query), otherwise the world grid; flavour 1 (>= 1)
+        # reads its query options from opt on every call, -1 once at construction
+        if is_frustum(opt):
+            self.querier = _frustum.lighting_fast_querier(device, opt)
+        elif int(getattr(opt, "wcoord_query", -1)) > 0:
+            self.querier = _worldcoords.lighting_fast_querier(device, opt)
+        else:
+            self.querier = lighting_fast_querier(device, opt)
 
     def set_points(self, points_xyz, points_embeding, points_color=None, points_dir=None, points_conf=None,
                    parameter=True, Rw2c=None, as_stored=False, **_):
