@@ -5,17 +5,29 @@ Same constructor (`lighting_fast_querier(device, opt)`), same `query_points(...)
 7-tuple of returns, same `clean_up()`, same `get_hyperparameters()` -- so that
 `NeuralPoints.__init__` (/root/reference/models/neural_points/neural_points.py:330-339) can pick
 this class up unchanged (see INTEGRATION.md).  Differences, all deliberate:
-  * the voxel grid is built once per point-cloud version and cached (the reference rebuilds it on
-    every ray chunk, query_worldcoords.cu:314-365);
+  * the voxel grid is built once per point cloud (storage object, address, version, size) and cached (the
+    reference rebuilds it on every ray chunk, query_worldcoords.cu:314-365);
   * ray positions are never materialised ([1,R,400,3] in the reference);
   * results are deterministic (canonical serial semantics, SURVEY.md 8a), overflow of max_o / P is
     reported (`last_grid_counters`) instead of resolved by wall-clock-seeded curand;
   * no CPU path: the CUDA library must be present, otherwise lib.load() raises.
 """
+import weakref
+
 import numpy as np
 import torch
 
 from . import lib as _lib
+
+
+def same_storage(ref, t):
+    """True when the weak reference `ref` (or None) points at the storage of tensor `t`.  The queriers cache their build on the points
+    they were handed, which arrive as a new tensor object on every call (NeuralPoints passes `self.xyz[None]`, the fused module a
+    detached `xyz`); every view and detached alias of one cloud shares its storage object, which lives exactly as long as the cloud's
+    memory.  A key of (data_ptr, _version, N) alone also matches a NEW cloud that the caching allocator placed where a freed one was
+    (both at version 0), which a feed-forward run (a new cloud from the network on every call) produces; its storage is another
+    object."""
+    return ref is not None and ref() is t.untyped_storage()
 
 
 def host_t_table(near, far, D):
@@ -166,6 +178,7 @@ class lighting_fast_querier():
         self.parity_slot0 = bool(getattr(self.opt, "pnb_parity_slot0", 1))
         self._grid = None
         self._grid_key = None
+        self._grid_storage = None   # weak reference to the storage of the grid's points (same_storage)
         self._hyper = None
         self._ws = None
         self._t_cache = {}
@@ -190,6 +203,7 @@ class lighting_fast_querier():
     def clean_up(self):
         self._grid = None
         self._grid_key = None
+        self._grid_storage = None
         self._hyper = None
         self._ws = None
         self.last_query = None
@@ -201,9 +215,10 @@ class lighting_fast_querier():
         return ranges_tensor, vsize_np, scaled_vdim_np
 
     def _grid_for(self, xyz):
-        """xyz: [N,3] contiguous fp32 on the device.  Rebuilt only when the point cloud changed."""
+        """xyz: [N,3] contiguous fp32 on the device.  Rebuilt only when the point cloud changed: another storage, address, version
+        or size."""
         key = (xyz.data_ptr(), xyz._version, xyz.shape[0], tuple(float(v) for v in self.opt.ranges) if self.opt.ranges is not None else None)
-        if self._grid is None or key != self._grid_key:
+        if self._grid is None or key != self._grid_key or not same_storage(self._grid_storage, xyz):
             vsize_np = self.opt.vsize
             ranges_tensor, scaled_vdim_np, _ = grid_hyperparameters(xyz[None], vsize_np, self.scaled_vsize_np, self.vscale_np,
                                                                     self.opt.kernel_size, self.opt.ranges)
@@ -212,6 +227,7 @@ class lighting_fast_querier():
             self._grid = VoxelGrid(xyz, ranges_np[:3], self.scaled_vsize_np, scaled_vdim_np, self.query_size, max_o,
                                    self.opt.P, parity_slot0=self.parity_slot0)
             self._grid_key = key
+            self._grid_storage = weakref.ref(xyz.untyped_storage())
             self.n_builds += 1
             self._hyper = (ranges_tensor, ranges_np, vsize_np, scaled_vdim_np)
             self.last_grid_counters = self._grid.counters

@@ -11,9 +11,10 @@ makes the reference's NeuralPoints use it unchanged (INTEGRATION.md).  Differenc
     (`last_build_counters`) instead of resolved by wall-clock-seeded curand or int8 wrap-around;
   * the build is cached per (points, camera, h, w, intrinsic, near, far, options), so the chunk loop over one view builds it once.
     The camera is compared by value; a call on a cached view synchronises once (for R').  The points are identified by the storage
-    and the autograd version of `point_xyz_w_tensor` (NeuralPoints passes `self.xyz[None]`): in-place updates through autograd-visible
-    ops and a new `self.xyz` Parameter rebuild, but a write through `.data` does not bump the version, and a freed cloud replaced by a
-    new tensor of the same shape at the same address looks unchanged.  After such an edit, call `clean_up()`;
+    object (a weak reference, point_query.same_storage), the address and the autograd version of `point_xyz_w_tensor` (NeuralPoints
+    passes `self.xyz[None]`): in-place updates through autograd-visible ops, a new `self.xyz` Parameter and a new cloud from a
+    feed-forward network (also one the caching allocator placed where the freed previous cloud was) rebuild, but a write through
+    `.data` does not bump the version.  After such an edit, call `clean_up()`;
   * only NN 2, inverse 0, B 1, K <= 8 and SR <= 128 (the DTU scripts' configuration) are implemented: anything else raises;
   * no pycuda and no CPU path: the CUDA library must be present, otherwise lib.load() raises.
 The jitter (`uniform`, `gaussian`) and `pers2w` are the reference's own torch expressions, so they round the same way.
@@ -21,10 +22,13 @@ The jitter (`uniform`, `gaussian`) and `pers2w` are the reference's own torch ex
 `run_fused` is the entry point of the fused module (pointnerf_b200.ray_marching with wcoord_query 0): the same query and tuple, handed
 to the shading kernels in the sample-compacted layout of pnb_frustum_samples.  Its one host synchronisation is the one that sizes R'.
 """
+import weakref
+
 import numpy as np
 import torch
 
 from . import lib as _lib
+from .point_query import same_storage
 
 
 def hyperparameters(opt, h, w, intrinsic, near_depth, far_depth):
@@ -98,13 +102,14 @@ class lighting_fast_querier():
         self.last_query_counters = None
         self.last_pixel_idx_cur = None
         self._key = None
+        self._storage = None     # weak reference to the storage of the build's points (same_storage)
         self._fr = None
         self._buf = None
         self._ws = None
         self._host = None
 
     def clean_up(self):
-        self._key = self._fr = self._buf = self._ws = None
+        self._key = self._storage = self._fr = self._buf = self._ws = None
 
     # ------------------------------------------------------------------ query_point_indices.py:50-73
     def get_hyperparameters(self, h, w, intrinsic, near_depth, far_depth):
@@ -118,7 +123,7 @@ class lighting_fast_querier():
         return radius_limit, depth_limit, ranges, vsize, vdim, scaled_vsize, scaled_vdim, vscale, range_gpu, scaled_vsize_gpu, \
             scaled_vdim_gpu, vscale_gpu, kernel_size_gpu, query_size_gpu
 
-    def _build(self, pers, n, key, ranges, scaled_vsize, scaled_vdim, vscale):
+    def _build(self, pers, n, key, storage, ranges, scaled_vsize, scaled_vdim, vscale):
         """The frustum build of this view (synchronises once, for its counters)."""
         lib = _lib.load()
         pts = pers[0, :n].to(torch.float32).contiguous()
@@ -135,7 +140,7 @@ class lighting_fast_querier():
                                          int(self.opt.max_o) if self.opt.max_o is not None else 0, int(self.opt.NN), int(self.inverse),
                                          stream, hc), "pnb_frustum_build")
         self.last_build_counters = {k: int(hc[i]) for k, i in _lib.FB.items()}
-        self._fr, self._key = fr, key
+        self._fr, self._key, self._storage = fr, key, weakref.ref(storage)
         self.n_builds += 1
 
     def _mask(self, pix, dev):
@@ -164,8 +169,8 @@ class lighting_fast_querier():
             raise NotImplementedError("pnb200: frustum query with batch size %d (only 1 is implemented)" % B)
         lib = _lib.load()
         dev = point_xyz_pers_tensor.device
-        # The build depends on the points (identified by storage and version, see the class docstring), the camera, the grid and the
-        # options.  The camera and the caller's point count live on the device: they are copied to pinned memory behind the work of
+        # The build depends on the points (identified by storage, address and version, see the module docstring), the camera, the grid
+        # and the options.  The camera and the caller's point count live on the device: they are copied to pinned memory behind the work of
         # this call and compared after the synchronisation that sizes R', so a call whose view is cached synchronises once.
         static = (point_xyz_w_tensor.data_ptr(), point_xyz_w_tensor._version, tuple(point_xyz_w_tensor.shape), int(h), int(w),
                   np.asarray(intrinsic).tobytes(), float(near_depth), float(far_depth), tuple(self.opt.vscale),
@@ -180,9 +185,10 @@ class lighting_fast_querier():
 
         def build():
             v = self._host.tolist()
-            self._build(point_xyz_pers_tensor, int(v[-1]), (static, tuple(v)), ranges, scaled_vsize, scaled_vdim, vscale)
+            self._build(point_xyz_pers_tensor, int(v[-1]), (static, tuple(v)), point_xyz_w_tensor.untyped_storage(), ranges,
+                        scaled_vsize, scaled_vdim, vscale)
 
-        if self._fr is None or self._key[0] != static:
+        if self._fr is None or self._key[0] != static or not same_storage(self._storage, point_xyz_w_tensor):
             torch.cuda.current_stream(dev).synchronize()       # a new view: the build needs the point count now
             build()
         ray_mask = self._mask(pix, dev)
