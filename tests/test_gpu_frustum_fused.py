@@ -11,16 +11,16 @@ reference's eager shading receives from that querier.
   gradients    the colour loss (plain background, or the model shell's bg_ray formula through coarse_is_background) plus the
                zero_one loss on conf_coefficient, against float64 autograd of the oracle with the backward's own LeakyReLU masks
                (as tests/test_gpu_grad_f64.py does: with 501 block1.0 inputs the BF16x3 recompute takes ~1e-5 of the masks on the
-               other side of zero, some 50 per step here, each moving one unit's row by up to ~5e-3 of scale), under the
-               bounded-outlier rule of tests/test_gpu_feat63.py
+               other side of zero, some 50 per step here, each moving one unit's row by up to ~5e-3 of scale), every point within
+               oracle/grad_check.RTOL with no outlier allowance, the MLP tensors within grad_check.FRUSTUM_MLP_RTOL, alpha_branch.0
+               with agg_intrp_order 1 within grad_check.ALPHA1_RTOL of its scale and ALPHA1_SUM_RTOL of each entry's sum |terms|
   whole frame  runner.render_image / probe_image bit for bit the 2304-ray chunk loops through forward(), with and without bg_ray,
                one build of the view; the probe outputs against oracle/probe_oracle.py in float64 within DESIGN §6's probe bounds
   bg_ray       for both queries, forward(bg_ray=...) is forward(bg_color=0) bit for bit, and the reference's fill_invalid on it is
                render_full(bg_ray=...) bit for bit
-No bound here is new: every one is an existing bound of DESIGN.md §6 or tests/test_gpu_feat63.py.  The file prints the errors it
+Every bound is one of DESIGN.md §6 or oracle/grad_check.py.  The file prints the errors it
 measures (pytest -s).
 """
-import ctypes
 import functools
 import json
 import os
@@ -30,8 +30,8 @@ import pytest
 import torch
 
 import frustum_shade_f64
-from oracle import forward_check, probe_oracle
-from pointnerf_b200 import harness, lib, runner, scene
+from oracle import grad_check, probe_oracle
+from pointnerf_b200 import harness, runner, scene
 from pointnerf_b200 import query_point_indices as qpi
 from pointnerf_b200.ray_marching import NeuralPoints, NeuralPointsRayMarching, PointAggregator, probe_keys
 
@@ -47,6 +47,7 @@ SAMPLE_BOUNDS = {"bf16x3": (1.8e-5, 6e-6), "bf16x3-general": (2e-5, 7e-6), "fp32
 PROBE_BOUNDS = dict(ray_max_far_dist=4.5e-7, shading_avg_color=5e-7, shading_avg_dir=6.5e-7, shading_avg_conf=6e-7,
                     shading_avg_embedding=4e-7)
 ZERO_EPS = 1e-3
+MLP_RTOL = grad_check.FRUSTUM_MLP_RTOL
 
 
 @functools.lru_cache(None)
@@ -202,25 +203,6 @@ def test_jitter_is_the_drop_ins():
 
 
 # ------------------------------------------------------------------------------------------------ gradients
-def _close(a, ref, name, rtol=3e-4):
-    a, ref = np.asarray(a, np.float64), np.asarray(ref, np.float64).reshape(np.asarray(a).shape)
-    scale = max(np.abs(ref).max(), 1e-6)
-    d = np.abs(a - ref).max()
-    assert d <= rtol * scale + 1e-7, "%s: max abs diff %.3e vs scale %.3e" % (name, d, scale)
-    return d / scale
-
-
-def _close_points(a, ref, name, rtol=3e-4, max_outlier_frac=0.01, outlier_rtol=2e-2):
-    """tests/test_gpu_feat63.py's rule: strict on all but <= 1 % of the points (LeakyReLU mask flips of the recompute), bounded on those."""
-    a, ref = np.asarray(a, np.float64)[0], np.asarray(ref, np.float64).reshape(np.asarray(a).shape)[0]
-    scale = max(np.abs(ref).max(), 1e-6)
-    d = np.abs(a - ref).max(axis=-1)
-    bad = d > rtol * scale + 1e-7
-    assert bad.sum() <= max(4, max_outlier_frac * d.shape[0]), "%s: %d of %d points beyond %.0e of scale" % (name, int(bad.sum()), d.shape[0], rtol)
-    assert d.max() <= outlier_rtol * scale, "%s: max abs diff %.3e vs scale %.3e" % (name, d.max(), scale)
-    return d.max() / scale, int(bad.sum())
-
-
 def _zero_one(cc):
     """The zero_one loss on conf_coefficient (models/base_rendering_model.py:629-641)."""
     val = torch.clamp(cc, ZERO_EPS, 1 - ZERO_EPS)
@@ -236,39 +218,14 @@ def _bg_ray(n, seed=11):
     return torch.rand((1, n, 3), generator=torch.Generator().manual_seed(seed)).to(DEV)
 
 
-def _kernel_slopes(net, q):
-    """The LeakyReLU masks the backward of the last training step took (its recompute buffers, pnb_backward_tables) as `slopes=` of
-    the oracle: pair rows in the flattened [R',SR,K] order of sample_pidx >= 0, colour rows per sample slot.  Candidate s of the frustum
-    query is entry s of the [R',SR] slots, and a valid sample's neighbours are its first K slots, so pair row (vi, k) is flat entry
-    valid_list[vi] * K + k."""
-    S, P = int(q.counters["n_valid"]), int(q.counters["n_pairs"])
-    out = (ctypes.c_void_p * 10)()
-    ws = net._bwd_ws
-    lib.check(lib.load().pnb_backward_tables(ws.data_ptr(), ws.numel(), S, q.desc.cap_samples, 63, out), "pnb_backward_tables")
-    dv = forward_check.dev_view
-    H = [dv(ws, out[0], torch.float32, (P, 256)), dv(ws, out[1], torch.float32, (P, 272))[:, :256],
-         dv(ws, out[2], torch.float32, (P, 256)), dv(ws, out[3], torch.float32, (P, 256))]
-    Cc = [dv(ws, out[i], torch.float32, (S, 128)) for i in (4, 5, 6)]
-    pair_off = dv(ws, out[7], torch.int32, (S + 1,)).long()
-    row_samp = dv(ws, out[8], torch.int32, (P,)).long()
-    vlist = dv(q.ws, q.desc.valid_list, torch.int32, (S,)).long()
-    flat = vlist[row_samp] * q.K + (torch.arange(P, device=row_samp.device) - pair_off[row_samp])
-    order = torch.argsort(flat)
-    slopes = [torch.where(h[order] > 0, 1.0, 0.01).double().cpu() for h in H]
-    for c in Cc:
-        sl = torch.ones(q.R2 * q.SR, 128, dtype=torch.float64)
-        sl[vlist.cpu()] = torch.where(c > 0, 1.0, 0.01).double().cpu()
-        slopes.append(sl)
-    return slopes
-
-
 def _grad_ref(net, tup, d, order, loss, slopes):
     """float64 autograd of the oracle on the drop-in's tuple, with the kernel's masks: the same loss, the gradients of every point
     group and MLP tensor."""
     pts = _points_cpu(net, grad=True)
     mlp = {k: v.detach().cpu().clone().requires_grad_(True) for k, v in net.aggregator.state_dict().items()}
     bg = (1.0, 1.0, 1.0) if loss == "color" else (0.0, 0.0, 0.0)
-    r = _shade64(net, tup, d, order, bg, pts=pts, mlp=mlp, slopes=slopes)
+    with frustum_shade_f64.recording_softplus() as rec:
+        r = _shade64(net, tup, d, order, bg, pts=pts, mlp=mlp, slopes=slopes)
     gt = _gt(int(tup[0].shape[1])).double()
     col = r["ray_color"]
     if loss == "bg_ray":
@@ -280,7 +237,8 @@ def _grad_ref(net, tup, d, order, loss, slopes):
     L = ((col - gt) ** 2).sum() + 1e-3 * _zero_one(cc)
     L.backward()
     return dict(emb=pts["embedding"].grad, color=pts["color"].grad, dir=pts["dir"].grad, conf=pts["conf"].grad,
-                mlp={k: v.grad for k, v in mlp.items()})
+                mlp={k: v.grad for k, v in mlp.items()},
+                abs_terms=frustum_shade_f64.alpha_branch_abs_terms(rec, r["hbar"]) if order == 1 else {})
 
 
 def _gt(n):
@@ -289,7 +247,7 @@ def _gt(n):
 
 @pytest.mark.parametrize("loss", ["color", "bg_ray"])
 @pytest.mark.parametrize("order", [2, 1])
-@pytest.mark.parametrize("precision,bwd_fp32", [("bf16x3", 0), ("bf16x3", 1), ("bf16x3", 4), ("fp32", 0)])
+@pytest.mark.parametrize("precision,bwd_fp32", [("bf16x3", 0), ("bf16x3", 1), ("bf16x3", 4), ("fp32", 0), ("fp32", 1)])
 def test_gradients_match_float64_autograd(precision, bwd_fp32, order, loss):
     mode = "bf16x3" if precision == "bf16x3" else "fp32"
     net, opt = _net(order=order, mode=mode, pnb_bwd_fp32=bwd_fp32)
@@ -305,18 +263,30 @@ def test_gradients_match_float64_autograd(precision, bwd_fp32, order, loss):
     L = ((col - _gt(col.shape[0]).to(DEV)) ** 2).sum() + 1e-3 * _zero_one(out["conf_coefficient"][0])
     L.backward()
     tup = _dropin(net, opt, d)
-    ref = _grad_ref(net, tup, d, order, loss, _kernel_slopes(net, net.last))
+    ref = _grad_ref(net, tup, d, order, loss, frustum_shade_f64.kernel_slopes(net, net.last))
     npn = net.neural_points
-    errs = {}
-    errs["emb"] = _close_points(npn.points_embeding.grad.cpu(), ref["emb"], "points_embeding")
-    errs["color"] = _close_points(npn.points_color.grad.cpu(), ref["color"], "points_color")
-    errs["dir"] = _close_points(npn.points_dir.grad.cpu(), ref["dir"], "points_dir")
-    errs["conf"] = _close(npn.points_conf.grad.cpu(), ref["conf"], "points_conf", rtol=1e-3)
-    worst = 0.0
-    for k, p in net.aggregator.named_parameters():
-        worst = max(worst, _close(p.grad.cpu(), ref["mlp"][k], "aggregator." + k, rtol=1e-3 if bwd_fp32 == 0 else 3e-4))
-    errs["mlp"] = worst
-    print("\n[frustum fused grads] %s/%d order %d %s: %s" % (precision, bwd_fp32, order, loss, errs))
+    rt = grad_check.RTOL[(bwd_fp32, precision)]
+    got = dict(emb=npn.points_embeding.grad.cpu(), color=npn.points_color.grad.cpu(), dir=npn.points_dir.grad.cpu())
+    errs = {k: float(grad_check.rel_point_errors(got[k], ref[k]).max()) for k in got}
+    params = dict(net.aggregator.named_parameters())
+    mlp = {k: grad_check.rel_error(p.grad.cpu(), ref["mlp"][k]) for k, p in params.items()}
+    alpha1 = {k: (mlp[k], grad_check.sum_error(params[k].grad.cpu(), ref["mlp"][k], t), float(t.max() / ref["mlp"][k].abs().max()))
+              for k, t in ref["abs_terms"].items()}
+    worst = max((v, k) for k, v in mlp.items() if k not in alpha1)
+    print("\n[frustum fused grads] %s/%d order %d %s: points %s | MLP worst %s %.2e%s" % (
+        precision, bwd_fp32, order, loss, " ".join("%s %.2e" % kv for kv in errs.items()), worst[1], worst[0],
+        "".join(" | %s %.2e of scale, %.2e of sum|terms| (sum|terms| %.0fx max|grad|)" % ((k,) + v) for k, v in alpha1.items())))
+    for k in got:
+        grad_check.check_points(got[k], ref[k], "points_" + k, rt[0])
+    grad_check.check_conf(npn.points_conf.grad.cpu(), ref["conf"], int((tup[0] <= 0).sum()), rt[0])
+    for k, e in mlp.items():
+        if k in alpha1:
+            continue
+        assert e <= MLP_RTOL[(bwd_fp32, precision)], "aggregator.%s: %.3e of scale > %.1e" % (k, e, MLP_RTOL[(bwd_fp32, precision)])
+    for k, (e, es, _) in alpha1.items():
+        b, bs = grad_check.ALPHA1_RTOL[precision], grad_check.ALPHA1_SUM_RTOL[(bwd_fp32, precision)]
+        assert e <= b, "aggregator.%s: %.3e of scale > %.1e" % (k, e, b)
+        assert es <= bs, "aggregator.%s: %.3e of sum |terms| > %.1e" % (k, es, bs)
     assert npn.xyz.grad is None
     net.check_errors()
 
