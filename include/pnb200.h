@@ -157,7 +157,7 @@ typedef struct {
 int pnb_version(void);
 const char* pnb_last_error(void);
 /* sizeof() of the POD structs as the library was compiled (0 grid, 1 query, 2 shade_opts, 3 mlp,
- * 4 points, 5 frustum) -- lets a foreign-language binding verify its mirror of the layout. */
+ * 4 points, 5 frustum, 6 vox) -- lets a foreign-language binding verify its mirror of the layout. */
 size_t pnb_struct_size(int which);
 
 /* ---- voxel grid ---- */
@@ -359,6 +359,42 @@ size_t pnb_frustum_samples_bytes(int R, int R2, int SR);
 int pnb_frustum_samples(pnb_query_t* q, void* ws, size_t ws_bytes, const int8_t* d_ray_mask, int R, int R2, int SR, int K,
                         const int32_t* d_sample_pidx, const float* d_sample_loc_w, const float* d_sample_loc,
                         const float* d_sample_ray_dirs, pnb_stream_t stream);
+
+/* ---- voxel down-sampling of a point cloud ----
+ * Replaces models/mvs/mvs_utils.py:484-561 (construct_vox_points{,_closest,_ind,_xyz}: torch.unique(dim=0) of the floored voxel
+ * indices, torch_scatter's scatter_mean and scatter_min) for pointnerf_b200.voxelize.  Results are canonical and identical from run to
+ * run: voxels in torch.unique's lexicographic order, a fixed fp64 reduction tree for the centroid, the lowest point index among tied
+ * residuals (DESIGN.md §5 "Voxel down-sampling"). */
+enum {                             /* counters written by pnb_vox_build (device int32[16] in its workspace) */
+    PNB_VC_N_VOX = 0,              /* M: occupied voxels */
+    PNB_VC_MAX_PTS = 1,            /* max points in one voxel */
+    PNB_VC_N_BIG = 2,              /* voxels of more than 256 points (reduced by a whole block) */
+    PNB_VC_N_OUT_OF_KEY = 3        /* points whose voxel index does not fit the key (the call fails) */
+};
+typedef struct {
+    int32_t n_points;              /* N */
+    int32_t key_bits;              /* 32 (10 bits per axis, indices in [0, 1024)) or 64 (21 bits, indices in [-2^20, 2^20)) */
+    int32_t n_vox;                 /* M */
+    int32_t n_big;                 /* counters[PNB_VC_N_BIG] */
+    const void* sorted_keys;       /* [N] uint32 | uint64, ascending */
+    const uint32_t* sorted_idx;    /* [N] point indices, voxel-major, ascending inside a voxel */
+    const uint32_t* seg_start;     /* [M+1] first sorted position of every voxel */
+    const uint32_t* big_list;      /* [n_big] voxels of more than 256 points */
+    int32_t* counters;             /* device int32[16], see PNB_VC_* */
+} pnb_vox_t;
+
+size_t pnb_vox_bytes(int N, int key_bits);
+/* Voxel of every point of d_xyz [N,3] (fp32): floorf((p - space_min) / vox_sz) per axis, an IEEE fp32 subtract and a true fp32 divide;
+ * d_space_min and d_vox_sz are device float[3].  Sorts, segments and, if d_inv_idx (int64 [N]) is given, writes every point's voxel.
+ * Synchronises the stream once, to return M in v->n_vox and the counters in h_counters (int32[16], required).  A voxel index outside
+ * the key's range: PNB_ERR_UNSUPPORTED.  v points into ws, which must outlive pnb_vox_outputs on it. */
+int pnb_vox_build(pnb_vox_t* v, void* ws, size_t ws_bytes, const float* d_xyz, int N, const float* d_space_min, const float* d_vox_sz,
+                  int key_bits, long long* d_inv_idx, pnb_stream_t stream, int32_t* h_counters);
+/* Per-voxel outputs of a pnb_vox_build, each optional: d_grid_idx int32 [M,3]; d_centroid fp32 [M,3], the mean of d_val [N,3] (fp32)
+ * over the voxel; d_min_idx int64 [M], the voxel's lowest point index, or with closest != 0 the point of d_val nearest its centroid.
+ * Nothing synchronises. */
+int pnb_vox_outputs(const pnb_vox_t* v, const float* d_val, int32_t* d_grid_idx, float* d_centroid, long long* d_min_idx, int closest,
+                    pnb_stream_t stream);
 
 #ifdef __cplusplus
 }

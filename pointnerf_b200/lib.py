@@ -60,10 +60,17 @@ class Frustum(C.Structure):
                 ("spts", C.c_void_p), ("col_list", C.c_void_p), ("col_far", C.c_void_p), ("counters", C.c_void_p)]
 
 
+class Vox(C.Structure):
+    _fields_ = [("n_points", C.c_int32), ("key_bits", C.c_int32), ("n_vox", C.c_int32), ("n_big", C.c_int32),
+                ("sorted_keys", C.c_void_p), ("sorted_idx", C.c_void_p), ("seg_start", C.c_void_p), ("big_list", C.c_void_p),
+                ("counters", C.c_void_p)]
+
+
 GC = dict(n_occ=0, max_pts=1, overflow_o=2, overflow_p=3, n_inrange=4, slot0_cell=5, first_pt=6)
 QC = dict(n_cand=0, n_valid=1, n_pairs=2, R1=3, R2=4, overflow=5)
 FB = dict(n_vox=0, max_pts=1, overflow_p=2, n_insert=3, n_occ=4, max_col_vox=5, overflow_o=6, max_col_samples=7, n_col_capped=8)
 FQ = dict(R2=0, n_bad_pixel=1)
+VC = dict(n_vox=0, max_pts=1, n_big=2, n_out_of_key=3)
 
 # every symbol include/pnb200.h declares (tests check that the .so exports all of them)
 SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes", "pnb_grid_build", "pnb_query_bytes", "pnb_query",
@@ -71,7 +78,8 @@ SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes",
            "pnb_mlp_pack_bytes", "pnb_mlp_pack", "pnb_point_pre_bytes", "pnb_point_pre", "pnb_shade_tc_bytes", "pnb_shade_forward_tc",
            "pnb_shade_tc_tables", "pnb_shade_tc_buffers", "pnb_backward_bytes", "pnb_shade_backward", "pnb_backward_tables", "pnb_aux_outputs",
            "pnb_aux_conf_backward", "pnb_probe_outputs", "pnb_frustum_bytes", "pnb_frustum_build", "pnb_frustum_query_bytes", "pnb_frustum_query",
-           "pnb_frustum_export", "pnb_frustum_samples_bytes", "pnb_frustum_samples", "pnb_composite_forward_bg_ray"]
+           "pnb_frustum_export", "pnb_frustum_samples_bytes", "pnb_frustum_samples", "pnb_composite_forward_bg_ray",
+           "pnb_vox_bytes", "pnb_vox_build", "pnb_vox_outputs"]
 # test-only library (csrc/selftest/pnb200_selftest.h)
 SELFTEST_LIB_PATH = os.path.join(_HERE, "csrc", "libpnb200_selftest.so")
 SELFTEST_SYMBOLS = ["pnb_selftest_last_error", "pnb_umma_selftest", "pnb_umma_selftest2", "pnb_gemm_tc_test"]
@@ -96,7 +104,7 @@ def load():
     lib.pnb_last_error.restype = C.c_char_p
     lib.pnb_struct_size.restype = C.c_size_t
     lib.pnb_struct_size.argtypes = [C.c_int]
-    for which, ty in enumerate((Grid, Query, ShadeOpts, Mlp, Points, Frustum)):
+    for which, ty in enumerate((Grid, Query, ShadeOpts, Mlp, Points, Frustum, Vox)):
         if lib.pnb_struct_size(which) != C.sizeof(ty):
             raise PnbError("ABI mismatch: struct %s is %d bytes in libpnb200.so, %d in the binding"
                            % (ty.__name__, lib.pnb_struct_size(which), C.sizeof(ty)))
@@ -180,6 +188,13 @@ def load():
     lib.pnb_frustum_samples.restype = C.c_int
     lib.pnb_frustum_samples.argtypes = [C.POINTER(Query), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.pnb_vox_bytes.restype = C.c_size_t
+    lib.pnb_vox_bytes.argtypes = [C.c_int, C.c_int]
+    lib.pnb_vox_build.restype = C.c_int
+    lib.pnb_vox_build.argtypes = [C.POINTER(Vox), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                  C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
+    lib.pnb_vox_outputs.restype = C.c_int
+    lib.pnb_vox_outputs.argtypes = [C.POINTER(Vox), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     _lib = lib
     return lib
 
