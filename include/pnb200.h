@@ -396,6 +396,27 @@ int pnb_vox_build(pnb_vox_t* v, void* ws, size_t ws_bytes, const float* d_xyz, i
 int pnb_vox_outputs(const pnb_vox_t* v, const float* d_val, int32_t* d_grid_idx, float* d_centroid, long long* d_min_idx, int closest,
                     pnb_stream_t stream);
 
+/* ---- plane background of bgmodel plane ----
+ * Replaces mvs_utils.get_rayplane_cross (models/mvs/mvs_utils.py:384-408) and the per-view work of MvsPointsVolumetricModel.set_bg
+ * (models/mvs_points_volumetric_model.py:272-310: homo_warp_nongrid, homo_warp_fg_mask + id2mask, extract_from_2d_grid's bilinear
+ * grid_sample, the +-0.03 plane-colour fit and the max over the views) for pointnerf_b200.plane_bg.  Every fp32 operation is rounded
+ * explicitly in the order csrc/plane_bg.cu documents (DESIGN.md §5 "Plane background").  Views: d_w2c [G,4,4] (world -> camera, row 3
+ * unread), d_K [G,3,3], d_hdwd int32 [G,2] (HD, WD: the bounds and the normalisation of the view), d_mask_off int64 [G] (offset of
+ * view g's foreground mask, int8 [HD,WD] row-major, in d_masks).  Nothing synchronises. */
+/* Ray / plane intersections d_xyz [R,3] of the rays d_raydir [R,3] from d_campos [3] with the plane through d_plane_pnt [3] of normal
+ * d_plane_normal [3]; (0, 0, 0) where n . d < 0.001f. */
+int pnb_plane_cross(const float* d_campos, const float* d_raydir, const float* d_plane_pnt, const float* d_plane_normal, int R,
+                    float* d_xyz, pnb_stream_t stream);
+/* Foreground masks of the points d_xyz [N,3]: zeroes d_masks (mask_bytes), then sets cell (ceil v, ceil u) of view g to 1 for every
+ * point that projects in bounds, without a depth test.  1 <= G <= 65535. */
+int pnb_plane_fg_masks(const float* d_xyz, int N, int G, const float* d_w2c, const float* d_K, const int32_t* d_hdwd,
+                       const long long* d_mask_off, int8_t* d_masks, size_t mask_bytes, pnb_stream_t stream);
+/* bg_ray d_bg [R,3] of the plane points d_xyz [R,3]: per view, the bilinear sample of d_img [G,3,H,W] (fp32) where the point projects
+ * in bounds onto a cell whose mask is < 1 and all three channels fit d_plane_color [3] +- 0.03, else 0; the max over the G views. */
+int pnb_plane_bg(const float* d_xyz, int R, int G, const float* d_w2c, const float* d_K, const int32_t* d_hdwd,
+                 const long long* d_mask_off, const int8_t* d_masks, const float* d_img, int H, int W, const float* d_plane_color,
+                 float* d_bg, pnb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -79,7 +79,7 @@ SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes",
            "pnb_shade_tc_tables", "pnb_shade_tc_buffers", "pnb_backward_bytes", "pnb_shade_backward", "pnb_backward_tables", "pnb_aux_outputs",
            "pnb_aux_conf_backward", "pnb_probe_outputs", "pnb_frustum_bytes", "pnb_frustum_build", "pnb_frustum_query_bytes", "pnb_frustum_query",
            "pnb_frustum_export", "pnb_frustum_samples_bytes", "pnb_frustum_samples", "pnb_composite_forward_bg_ray",
-           "pnb_vox_bytes", "pnb_vox_build", "pnb_vox_outputs"]
+           "pnb_vox_bytes", "pnb_vox_build", "pnb_vox_outputs", "pnb_plane_cross", "pnb_plane_fg_masks", "pnb_plane_bg"]
 # test-only library (csrc/selftest/pnb200_selftest.h)
 SELFTEST_LIB_PATH = os.path.join(_HERE, "csrc", "libpnb200_selftest.so")
 SELFTEST_SYMBOLS = ["pnb_selftest_last_error", "pnb_umma_selftest", "pnb_umma_selftest2", "pnb_gemm_tc_test"]
@@ -195,6 +195,12 @@ def load():
                                   C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
     lib.pnb_vox_outputs.restype = C.c_int
     lib.pnb_vox_outputs.argtypes = [C.POINTER(Vox), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    lib.pnb_plane_cross.restype = C.c_int
+    lib.pnb_plane_cross.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_void_p]
+    lib.pnb_plane_fg_masks.restype = C.c_int
+    lib.pnb_plane_fg_masks.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
+    lib.pnb_plane_bg.restype = C.c_int
+    lib.pnb_plane_bg.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int] + [C.c_void_p] * 3
     _lib = lib
     return lib
 
