@@ -25,6 +25,11 @@ U32 = 2.0 ** -24    # unit roundoff of fp32
 # MLP 3.5e-6 (both in raydist_mode_unit 0 at SR 80).
 # The tensor-core dX / dW GEMMs carry the ~1e-5 of the BF16x3 split (tests/test_gpu_umma.py); in mode 1 the points see the BF16x3
 # forward's (sigma, rgb), from which the composite backward starts.  One flipped or lost pair row moves its points by ~1e-3 of scale.
+# The exact-count cases (batches of 1 to 2049 valid samples or 1 to 4097 pair rows, S_TARGETS / P_TARGETS; H100 80GB HBM3 at 700 W)
+# measured at most: mode 0 points 3.0e-5, MLP 2.0e-5 (fp32 forward 1.0e-5, 1.7e-5); mode 4 points 3.3e-5, MLP 2.1e-5; mode 1 points
+# 1.9e-6, MLP 3.2e-6 (fp32 forward 6.0e-7, 2.7e-6).  The largest tensor-core errors are one-ray batches whose every valid sample has
+# a single neighbour (S = P = 8 and 9): each point's gradient comes from one pair row, so nothing averages the BF16x3 error of its
+# chain of GEMMs down.
 RTOL = {(0, "bf16x3"): (4e-5, 1.2e-4), (0, "fp32"): (4e-5, 1.2e-4), (4, "bf16x3"): (4e-5, 1.2e-4),
         (1, "bf16x3"): (2e-5, 5e-6), (1, "fp32"): (2e-6, 3e-6)}
 
@@ -119,6 +124,97 @@ class MaskRecorder:
 def flipped_rows(slopes_a, slopes_b):
     """Per layer, the rows in which some unit has a different slope in the two mask sets."""
     return [(sa != sb).any(dim=-1) for sa, sb in zip(slopes_a, slopes_b)]
+
+
+# Batch sizes at which the backward's launch geometry changes (backward.cu, gemm_tc.cu), as exact counts of valid samples S (n_valid)
+# and of pair rows P (n_pairs):
+#   S: one warp per valid sample, 8 per block (k_bwd_build, k_bwd_reduce_fwd / _bwd): 1, 8, 9; 128-row output tiles of the colour GEMMs
+#      (M = S): 127, 128, 129; 256-row slabs of k_bwd_head, k_dw_small<3>, k_bwd_alpha_params_o1: 255, 256, 257; 512-row slabs of
+#      k_colsum4: 511, 512, 513; blocks of 1024 of exclusive_scan_u32 over the per-sample pair counts: 1024, 1025; the colour dW
+#      split-K (max(2, ceil(S / 2048)) splits) and 2048-row slabs of k_colsum / k_gemm<true>: 2048, 2049
+#   P: the dW split-K's single-split fallback (kchunk rounded up to 32): 1, 32, 33; 128-row tiles of the pair GEMMs (M = P): 127, 128,
+#      129; 256-row slabs of k_bwd_alpha_params: 255, 256, 257; split-K and 2048-row slabs: 2047, 2048, 2049, 4096, 4097
+S_TARGETS = (1, 8, 9, 127, 128, 129, 255, 256, 257, 511, 512, 513, 1024, 1025, 2048, 2049)
+P_TARGETS = (1, 32, 33, 127, 128, 129, 255, 256, 257, 2047, 2048, 2049, 4096, 4097)
+SPLITK_ROWS, SPLITK_MAX = 2048, 64
+
+
+def dw_splits(rows):
+    """(splits gemm_tn_acc asks for, splits gemm_tc runs) of a dW GEMM over `rows` reduction rows: max(2, ceil(rows / 2048)) capped at
+    64, then kchunk = that share rounded up to 32 rows and the count recomputed (1 for 1..32 rows: one split through the workspace)."""
+    asked = min(max(2, -(-rows // SPLITK_ROWS)), SPLITK_MAX)
+    kchunk = -(-(-(-rows // asked)) // 32) * 32
+    return asked, -(-rows // kchunk)
+
+
+def ray_census(sample_pidx, ray_mask):
+    """Per hit ray of a query (sample_pidx [R',SR,K] of the hit rays, ray_mask [R]): its index among the R rays, its valid samples (slots
+    with a neighbour: the rows of n_valid) and its pairs (filled K slots: the rows of n_pairs)."""
+    v = np.asarray(sample_pidx) >= 0
+    return dict(rays=np.nonzero(np.asarray(ray_mask))[0], S=v.any(-1).sum(-1), P=v.sum((-2, -1)))
+
+
+def select_rays(counts, target):
+    """Positions (ascending) of entries of counts [n] (non-negative integers) that sum to `target` exactly, or None if no subset does.
+    Subset-sum over the prefix of the entries it needs: among the subsets, the one that skips every entry it can from the back, so
+    that a target reached by a prefix of the rays takes that prefix."""
+    c = np.asarray(counts, np.int64)
+    if target < 0 or target > int(c.sum()):
+        return None
+    n = int(np.searchsorted(np.cumsum(c), target)) + 1 if target > 0 else 0
+    while True:
+        n = min(n, len(c))
+        reach = np.zeros((n + 1, target + 1), bool)        # reach[i][s]: some subset of the first i entries sums to s
+        reach[0, 0] = True
+        for i in range(n):
+            reach[i + 1] = reach[i]
+            if c[i] <= target:
+                reach[i + 1, c[i]:] |= reach[i, :target + 1 - c[i]]
+        if reach[n, target] or n == len(c):
+            break
+        n *= 2
+    if not reach[n, target]:
+        return None
+    pick, s = [], target
+    for i in range(n, 0, -1):
+        if not reach[i - 1, s]:
+            pick.append(i - 1)
+            s -= int(c[i - 1])
+    return np.array(pick[::-1], np.int64)
+
+
+_CENSUS = {}
+
+
+def frame_census(cfg_name, rotated=False, device="cuda:0", **over):
+    """ray_census of the whole frame of scene.CONFIGS[cfg_name] (camera scene.orbit_rotation() if rotated, query options `over` of
+    harness.make_opt), from the drop-in's own query export, plus the pixel of every hit ray.  Cached per arguments."""
+    key = (cfg_name, rotated, device, tuple(sorted(over.items())))
+    if key not in _CENSUS:
+        from pointnerf_b200 import harness, scene
+        from pointnerf_b200.point_query import make_cam_opts
+        cfg = scene.CONFIGS[cfg_name]
+        net, _, _ = harness.build_model(cfg, device, **over)
+        rays = scene.make_rays(cfg, None, camrotc2w=scene.orbit_rotation() if rotated else None)
+        r = {k: v.to(device) for k, v in rays.items()}
+        with torch.no_grad():
+            net(r["campos"], r["raydir"], bg_color=r["bg_color"], camrotc2w=r["camrotc2w"], pixel_idx=r["pixel_idx"], near=r["near"],
+                far=r["far"], h=r["h"], w=r["w"], intrinsic=r["intrinsic"])
+        net.check_errors()
+        q = net.last
+        ex = q.export(make_cam_opts(list(q.desc.campos), rays["camrotc2w"][0]), want_pers=False, want_dirs=False)
+        c = ray_census(ex["sample_pidx"].cpu().numpy(), ex["ray_mask"].cpu().numpy())
+        assert int(c["S"].sum()) == int(q.counters["n_valid"]) and int(c["P"].sum()) == int(q.counters["n_pairs"])
+        c["pixels"] = rays["pixel_idx"][0].numpy()[c["rays"]]
+        _CENSUS[key] = c
+    return _CENSUS[key]
+
+
+def pixels_for(census, count, target):
+    """The pixels of a subset of the census's hit rays whose valid samples (count "S") or pairs (count "P") add up to target exactly."""
+    pick = select_rays(census[count], target)
+    assert pick is not None, "no subset of the frame's hit rays has %s = %d (the frame holds %d)" % (count, target, int(census[count].sum()))
+    return census["pixels"][pick]
 
 
 def kernel_masks(net, q, F, camrotc2w):

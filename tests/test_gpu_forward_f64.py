@@ -34,7 +34,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import forward_check, shade_oracle, shade_oracle_rw2c
+from oracle import forward_check, grad_check, shade_oracle, shade_oracle_rw2c
 from pointnerf_b200 import harness, lib, scene
 from pointnerf_b200.point_query import make_cam_opts
 
@@ -320,3 +320,16 @@ def test_checkpoint_value_ranges(kernel, what):
         assert float(npn.points_color.min()) < -0.4 and float(npn.points_color.max()) > 1.4
     else:
         assert float(npn.points_embeding.abs().max()) > (6.0 if what == "embedding_x4" else 15.0)
+
+
+# ---- F. tile boundaries: batches of exactly 127, 128 or 129 pair rows (the 128-row tile of k_shade_wg) or valid samples (the colour
+# ---- tile of k_color_wg), a subset of the tiny frame's hit rays whose counts add up to the target (grad_check.pixels_for)
+@pytest.mark.parametrize("count,target", [(c, t) for c in ("P", "S") for t in (127, 128, 129)])
+@pytest.mark.parametrize("F", [32, 63])
+@pytest.mark.parametrize("kernel", ["frozen", "general"])
+def test_tile_boundaries(kernel, F, count, target):
+    pixels = grad_check.pixels_for(grad_check.frame_census("tiny", rotated=True, device=DEV), count, target)
+    net, _, smap = _run("tiny", 0, F=F, kernel=kernel, pixels=pixels)
+    S, P = smap["cand"].shape[0], int(net.last.counters["n_pairs"])
+    print("[fwd-f64 exact] %s = %d: rays=%d S=%d P=%d" % (count, target, len(pixels), S, P))
+    assert (S if count == "S" else P) == target, "the batch is off its boundary: S=%d P=%d" % (S, P)

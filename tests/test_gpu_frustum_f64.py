@@ -367,8 +367,22 @@ GRAD_CASES = [("layers", "translucent"), ("dtu_surface_limits", "translucent"), 
 @pytest.mark.parametrize("precision,mode", [("bf16x3", 0), ("bf16x3", 4), ("bf16x3", 1), ("fp32", 0), ("fp32", 1)])
 @pytest.mark.parametrize("name,bias_name", GRAD_CASES, ids=["%s-%s" % c for c in GRAD_CASES])
 def test_gradients_match_float64_autograd(name, bias_name, precision, mode, order):
+    _gradient_case(name, bias_name, precision, mode, order)
+
+
+@pytest.mark.parametrize("precision,mode", [("bf16x3", 0), ("bf16x3", 4), ("bf16x3", 1)])
+def test_gradients_one_hit_ray(precision, mode):
+    """A batch of one hit ray (the centre pixel of layers: 14 valid samples on three surfaces): k_bwd_build<..., XSAMP> with one warp
+    busy, and every backward GEMM and slab on one partial tile or slab, against float64 as above."""
+    q = _gradient_case("layers", "translucent", precision, mode, 2, pixels=np.array([[80, 60]], np.int32))
+    assert q.R2 == 1 and 8 < int(q.counters["n_valid"]) < 128, (q.R2, int(q.counters["n_valid"]))
+
+
+def _gradient_case(name, bias_name, precision, mode, order, pixels=None):
+    """One training step of the frustum module on the scene's pixels (or `pixels`), its gradients against float64 autograd with the
+    backward's own masks.  Returns the query."""
     net, opt = _net(name, BIAS[bias_name], order, "fp32" if precision == "fp32" else "general", is_train=True, pnb_bwd_fp32=mode)
-    d = _data(name, _pixels(name), None)
+    d = _data(name, _pixels(name) if pixels is None else pixels, None)
     R = d["pixel_idx"].shape[1]
     g = torch.Generator().manual_seed(3)
     bg_ray = torch.rand((1, R, 3), generator=g)
@@ -421,3 +435,4 @@ def test_gradients_match_float64_autograd(name, bias_name, precision, mode, orde
     for k, e in mlp_errs.items():
         assert e <= b_mlp, "aggregator.%s: %.3e > %.1e" % (k, e, b_mlp)
     assert npn.xyz.grad is None
+    return q

@@ -135,7 +135,7 @@ def _run_case(cfg_name, side, F=32, frames=False, order=2, mode=0, precision="bf
         assert v <= rtol, "%s: %.3e of scale > %.1e" % (k, v, rtol)
     assert err0[0] <= err0[1], "points_conf of point 0: %.3e > %.3e" % err0
     assert npn.xyz.grad is None
-    return P, flips, dict(net=net, n_long=n_long, n_sat=n_sat, hit=hit)
+    return P, flips, dict(net=net, n_long=n_long, n_sat=n_sat, hit=hit, S=int(q.counters["n_valid"]))
 
 
 @pytest.mark.parametrize("mode", [0, 4, 1])
@@ -150,6 +150,50 @@ def test_backward_matches_float64_with_kernel_masks(F, frames, order, mode, monk
 @pytest.mark.parametrize("F", [32, 63])
 def test_fp32_forward_backward_matches_float64(F, mode, monkeypatch):
     _run_case("tiny", 20, F=F, mode=mode, precision="fp32", monkeypatch=monkeypatch)
+
+
+# ---- batches of exactly S valid samples or P pair rows on either side of each point where the backward's launch geometry changes
+# ---- (grad_check.S_TARGETS / P_TARGETS): the pixels are a subset of the tiny frame's hit rays whose counts add up to the target
+def _exact_case(count, target, F, mode, monkeypatch, order=2, precision="bf16x3", **over):
+    census = grad_check.frame_census("tiny", device=DEV, **over)
+    pixels = grad_check.pixels_for(census, count, target)
+    P, _, info = _run_case("tiny", 0, F=F, order=order, mode=mode, precision=precision, pixels=pixels, monkeypatch=monkeypatch, **over)
+    S = info["S"]
+    if mode == 1:       # the CUDA-core dW tiles: one atomic z-slice per 2048 rows
+        splits = "k_gemm<true> slices S %d P %d" % (-(-S // grad_check.SPLITK_ROWS), -(-P // grad_check.SPLITK_ROWS))
+    else:               # (asked, run) of the tensor-core split-K
+        splits = "split-K S %s P %s" % (grad_check.dw_splits(S), grad_check.dw_splits(P))
+    print("[grad-f64 exact] %s = %d: rays=%d S=%d P=%d dW %s" % (count, target, len(pixels), S, P, splits))
+    assert (S if count == "S" else P) == target, "the batch is off its boundary: S=%d P=%d" % (S, P)
+    return S, P
+
+
+@pytest.mark.parametrize("target", grad_check.S_TARGETS)
+@pytest.mark.parametrize("mode", [0, 4, 1])
+@pytest.mark.parametrize("F,order", [(32, 2), (63, 2), (32, 1)])
+def test_exact_valid_sample_counts(F, order, mode, target, monkeypatch):
+    _exact_case("S", target, F, mode, monkeypatch, order=order)
+
+
+@pytest.mark.parametrize("target", grad_check.P_TARGETS)
+@pytest.mark.parametrize("mode", [0, 4, 1])
+@pytest.mark.parametrize("F", [32, 63])
+def test_exact_pair_row_counts(F, mode, target, monkeypatch):
+    _exact_case("P", target, F, mode, monkeypatch)
+
+
+@pytest.mark.parametrize("mode", [0, 4, 1])
+@pytest.mark.parametrize("F", [32, 63])
+def test_one_sample_one_pair(F, mode, monkeypatch):
+    """SR 1, K 1: every hit ray holds one valid sample with one neighbour, so one ray is S = P = 1."""
+    S, P = _exact_case("S", 1, F, mode, monkeypatch, SR=1, K=1)
+    assert P == 1
+
+
+@pytest.mark.parametrize("count,target", [("S", 1), ("S", 128), ("S", 2049), ("P", 1), ("P", 33), ("P", 129), ("P", 4097)])
+@pytest.mark.parametrize("mode", [0, 1])
+def test_exact_counts_fp32_forward(mode, count, target, monkeypatch):
+    _exact_case(count, target, 32, mode, monkeypatch, precision="fp32")
 
 
 @pytest.mark.parametrize("mode", [0, 4, 1])

@@ -2,6 +2,7 @@
 import pytest
 import torch
 
+from oracle import grad_check
 from pointnerf_b200 import lib as _lib
 
 pytestmark = pytest.mark.gpu
@@ -69,17 +70,22 @@ def test_wgmma_cluster_pair(mode, K, N):
 
 # ---- the wgmma GEMM engine of the backward pass (csrc/gemm_tc.cu) against fp64 matmuls, every operand form it is used in
 def _gemm_tc(A, a_rs, a_ks, B, b_rs, b_ks, M, N, K, ldc, bias=None, act=0, dact=None, ldd=0, dact_n=0, splits=1, C0=None, precise=0):
+    """C [M x ldc] (C0, or 7.0 everywhere) with 128 guard rows of 7.0 below it that must stay untouched; the split-K workspace starts
+    as NaN, so that a partial tile that is not written shows."""
     l = _lib.load_selftest()
-    C = torch.full((M, ldc), 7.0, device="cuda") if C0 is None else C0.clone()
+    C = torch.full((M + 128, ldc), 7.0, device="cuda")
+    if C0 is not None:
+        C[:M] = C0
     err = torch.zeros(4, dtype=torch.int32, device="cuda")
-    part = torch.empty(max(max(splits, 1) * M * N, 1 << 19), device="cuda")
+    part = torch.full((max(max(splits, 1) * M * N, 1 << 19),), float("nan"), device="cuda")
     ptr = lambda t: t.data_ptr() if t is not None else None
     _lib.check_selftest(l.pnb_gemm_tc_test(A.data_ptr(), a_rs, a_ks, B.data_ptr(), b_rs, b_ks, C.data_ptr(), ldc, M, N, K, ptr(bias), act,
                                            ptr(dact), ldd, dact_n, splits, part.data_ptr(), part.numel() * 4, 1 if C0 is not None else 0,
                                            precise, err.data_ptr(), torch.cuda.current_stream().cuda_stream), "pnb_gemm_tc_test")
     torch.cuda.synchronize()
     assert int(err[0]) == 0
-    return C
+    assert torch.all(C[M:] == 7.0), "rows beyond M written"
+    return C[:M]
 
 
 def _rel(a, ref):
@@ -87,7 +93,10 @@ def _rel(a, ref):
 
 
 @pytest.mark.parametrize("M,N,K", [(300, 256, 288), (128, 128, 128), (1000, 256, 272), (77, 288, 256), (4096, 128, 128),
-                                   (1000, 256, 512)])   # F = 63: the 512-wide block1.0 recompute (its NT: 512 output columns)
+                                   (1000, 256, 512),    # F = 63: the 512-wide block1.0 recompute (its NT: 512 output columns)
+                                   # one row, and either side of the 64-row warpgroup half and of the 128-row tile
+                                   (1, 256, 288), (2, 256, 272), (63, 128, 128), (64, 256, 288), (65, 128, 272), (127, 288, 256),
+                                   (129, 256, 272)])
 def test_gemm_tc_nn_nt(M, N, K):
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     X = torch.randn(M, K + 16, device="cuda", generator=g)[:, :K]                 # leading dimension != K
@@ -98,7 +107,9 @@ def test_gemm_tc_nn_nt(M, N, K):
     H = _gemm_tc(X, lda, 1, Wt, 1, N, M, N, K, N + 16, bias=bias, act=1)
     ref = torch.nn.functional.leaky_relu(X.double() @ Wt.double() + bias.double(), 0.01)
     assert _rel(H[:, :N], ref) < 2e-5 and torch.all(H[:, N:] == 7.0)
-    # the 3-part split (6 products): stops at ~1e-6 - the tensor core does not accumulate with full fp32 precision
+    # the 3-part split (6 products): stops at ~1e-6 - the tensor core does not accumulate with full fp32 precision.  Its error grows
+    # linearly with K, not with M: over M of 1 to 1000 and four seeds, at most 1.2e-6 at K 128, 2.5e-6 at K 256 to 288 and 4.6e-6
+    # at K 512 (H100 80GB HBM3, 700 W), so that the bound below holds K 512 on this test's seed of (1000, 256, 512) only
     Hp = _gemm_tc(X, lda, 1, Wt, 1, N, M, N, K, N + 16, bias=bias, act=1, precise=1)
     assert _rel(Hp[:, :N], ref) < 4e-6, _rel(Hp[:, :N], ref)      # ~1e-6: the accumulation precision of the tensor core, not fp32
     # NT (dX = dZ W * LeakyReLU'(Y)): A = dZ [M x N], B(n=k_in, k=n_out) = Wt[k_in*N + n_out]; result [M x K]
@@ -133,9 +144,16 @@ def test_gemm_tc_nt_partial_n_tile(dact):
 @pytest.mark.parametrize("rows,Kin,Nout,splits", [(5000, 288, 256, 3), (130000, 256, 256, 64), (999, 128, 128, 2), (40000, 272, 256, 20),
                                                   # F = 63 block1.0 dW (Kin 512) at the backward's split counts: the 2-split
                                                   # clamp, (rows + 2047) / 2048, and the 64-split cap
-                                                  (3000, 512, 256, 2), (40000, 512, 256, 20), (130000, 512, 256, 64)])
+                                                  (3000, 512, 256, 2), (40000, 512, 256, 20), (130000, 512, 256, 64)] +
+                         # the reduction rows of a small batch at gemm_tn_acc's split count: 1..32 rows run one split (kchunk 32)
+                         # through the workspace, 33 leaves the second split one row, and either side of the 2048-row slabs
+                         [(r, kin, nout, grad_check.dw_splits(r)[0]) for r, kin, nout in (
+                             (1, 288, 128), (2, 128, 128), (31, 256, 256), (32, 272, 256), (33, 512, 256), (2047, 256, 256),
+                             (2048, 288, 128), (2049, 272, 256), (4097, 512, 256))])
 def test_gemm_tc_tn_splitk_accumulate(rows, Kin, Nout, splits):
     """dWt[Kin x Nout] += X^T dZ: both operands transposed on the way into shared memory, deterministic split-K, accumulation."""
+    assert splits == grad_check.dw_splits(rows)[0], "not the split count the backward passes"
+    print("\n[gemm_tc tn] rows=%d Kin=%d Nout=%d splits (asked, run) %s" % (rows, Kin, Nout, grad_check.dw_splits(rows)))
     g = torch.Generator(device="cuda").manual_seed(rows)
     X = torch.randn(rows, Kin, device="cuda", generator=g)
     dZ = torch.randn(rows, Nout + 16, device="cuda", generator=g)[:, :Nout]
@@ -143,5 +161,6 @@ def test_gemm_tc_tn_splitk_accumulate(rows, Kin, Nout, splits):
     out = _gemm_tc(X, 1, Kin, dZ, 1, dZ.stride(0), Kin, Nout, rows, Nout, splits=splits, C0=C0)
     ref = C0.double() + X.double().t() @ dZ.double()
     assert _rel(out, ref) < 2e-5
+    assert _rel(out.double() - C0.double(), ref - C0.double()) < 2e-5                # the product alone: not hidden by C0's scale
     out2 = _gemm_tc(X, 1, Kin, dZ, 1, dZ.stride(0), Kin, Nout, rows, Nout, splits=splits, C0=C0)
     assert torch.equal(out, out2)                                                   # deterministic (no atomics)

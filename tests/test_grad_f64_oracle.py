@@ -154,3 +154,54 @@ def test_backward_defects_need_a_coloured_background_and_varying_conf_weights(go
                 check()
         else:
             check()
+
+
+# ---- the exact-count pixel selection of tests/test_gpu_grad_f64.py / test_gpu_forward_f64.py, on the C query oracle's census
+def _oracle_census(rotated, pixels=None, **over):
+    from oracle import pipeline, query_oracle
+    from pointnerf_b200 import harness
+    cfg = scene.CONFIGS["tiny"]
+    opt = harness.make_opt(cfg, **over)
+    pts = scene.make_points(cfg)
+    rays = scene.make_rays(cfg, pixels, camrotc2w=scene.orbit_rotation() if rotated else None)
+    rng6, svs, dim = pipeline.hyperparameters(pts["xyz"], opt.vsize, opt.vscale, opt.kernel_size, opt.ranges)
+    o = query_oracle.query(pts["xyz"].numpy(), rng6[:3], svs, dim, opt.kernel_size, opt.query_size, pts["xyz"].shape[0], opt.P,
+                           float(pipeline.radius_limit(opt.radius_limit_scale, opt.vsize)), campos=rays["campos"][0].numpy(),
+                           raydir=rays["raydir"][0].numpy(), t=pipeline.t_table(cfg.near, cfg.far, cfg.D), SR=opt.SR, K=opt.K)
+    c = grad_check.ray_census(o["sample_pidx"], o["ray_mask"])
+    c["pixels"] = rays["pixel_idx"][0].numpy()[c["rays"]]
+    return c, o["counters"]
+
+
+@pytest.mark.parametrize("rotated", [False, True])
+def test_exact_count_selection_on_the_query_oracle(rotated):
+    """Every S and P target is hit exactly by a subset of the tiny frame's hit rays, and the C oracle queried on just those pixels counts
+    the same S or P (rays are independent); SR 1, K 1 gives S = P = 1 from one hit ray."""
+    c, counters = _oracle_census(rotated)
+    assert int(c["S"].sum()) == counters["n_valid_samples"] and int(c["P"].sum()) == counters["n_valid_pairs"]
+    for count, targets in (("S", grad_check.S_TARGETS), ("P", grad_check.P_TARGETS)):
+        for target in targets:
+            pick = grad_check.select_rays(c[count], target)
+            assert pick is not None and int(c[count][pick].sum()) == target, (count, target)
+            assert np.all(np.diff(pick) > 0)
+            _, sub = _oracle_census(rotated, c["pixels"][pick])
+            assert sub["R2"] == len(pick) and sub["n_valid_samples" if count == "S" else "n_valid_pairs"] == target, (count, target, sub)
+    c1, _ = _oracle_census(rotated, K=1, SR=1)
+    _, sub = _oracle_census(rotated, grad_check.pixels_for(c1, "S", 1), K=1, SR=1)
+    assert sub["R2"] == 1 and sub["n_valid_samples"] == sub["n_valid_pairs"] == 1
+
+
+def test_selection_reports_an_unreachable_target():
+    c, _ = _oracle_census(False)
+    assert grad_check.select_rays(c["P"], int(c["P"].sum()) + 1) is None
+    assert grad_check.select_rays(c["P"], int(c["P"].sum())).tolist() == list(range(len(c["P"])))
+    assert grad_check.select_rays([2, 4, 6, 8], 5) is None and grad_check.select_rays([2, 4, 6, 8], 14).tolist() == [0, 1, 3]
+    assert grad_check.select_rays([3, 0, 5], 0).tolist() == []
+    with pytest.raises(AssertionError, match="no subset"):
+        grad_check.pixels_for(dict(S=np.array([2, 4]), pixels=np.zeros((2, 2))), "S", 3)
+
+
+def test_dw_split_counts():
+    """gemm_tn_acc's split count and gemm_tc's recomputed one at the row counts the backward cases aim at."""
+    got = {r: grad_check.dw_splits(r) for r in (1, 32, 33, 2048, 2049, 4096, 4097, 130000)}
+    assert got == {1: (2, 1), 32: (2, 1), 33: (2, 2), 2048: (2, 2), 2049: (2, 2), 4096: (2, 2), 4097: (3, 3), 130000: (64, 64)}
