@@ -639,19 +639,19 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
                 "pnb_shade_backward: null argument");
     PNB_REQUIRE(d_ray_color || d_opacity || d_bg_T, PNB_ERR_INVALID,
                 "pnb_shade_backward: no upstream gradient (d_ray_color, d_opacity and d_bg_T are all NULL)");
-    int F = 0;
-    { const int rc = feat_check(pts, mlp, "pnb_shade_backward", &F); if (rc) return rc; }
-    const int KP1 = kpad1_of(F);
+    Variant v;
+    { const int rc = resolve_variant("pnb_shade_backward", pts, mlp, q, XsRule::frames, &v); if (rc) return rc; }
+    const int F = v.F, KP1 = kpad1_of(F);
     Layout L = carve(ws, ws_bytes, n_valid, q->cap_samples, F);
     PNB_REQUIRE(L.bytes <= ws_bytes, PNB_ERR_WORKSPACE, "pnb_shade_backward: workspace %zu < required %zu", ws_bytes, L.bytes);
     // composite backward first (also covers n_valid == 0)
     CompBwdParams cp;
     cp.q = *q; cp.o = *opts; cp.sigma_rgb = (const float4*)d_sigma_rgb_fwd; cp.d_ray_color = d_ray_color; cp.d_sigma_rgb = L.d_sigma_rgb;
     cp.d_opacity = d_opacity; cp.d_bg_T = d_bg_T;
-    const bool xs = q->xs_loc_w != nullptr;                  // explicit samples (the frustum query)
-    { const int rc = xs_check(q, pts, F, "pnb_shade_backward"); if (rc) return rc; }
-    void (*comp)(CompBwdParams) = d_ray_color && !d_opacity && !d_bg_T ? (xs ? k_composite_bwd<false, true> : k_composite_bwd<false>)   // colour-only loss
-                                                                       : (xs ? k_composite_bwd<true, true> : k_composite_bwd<true>);
+    const bool colour_only = d_ray_color && !d_opacity && !d_bg_T;   // colour-only loss
+    const auto comp = with_bool(!colour_only, [&](auto EXT) {
+        return with_bool(v.xs, [&](auto XS) { return k_composite_bwd<EXT, XS>; });
+    });
     comp<<<(q->R + 127) / 128, 128, 0, st>>>(cp);
     if (n_valid <= 0) { PNB_CHECK_CUDA(cudaGetLastError()); return PNB_OK; }
     PNB_REQUIRE(n_pairs >= n_valid && n_pairs <= n_valid * PNB_MAX_K, PNB_ERR_INVALID, "pnb_shade_backward: n_pairs %d inconsistent with n_valid %d", n_pairs, n_valid);
@@ -669,10 +669,7 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     GemmCtx cx{(flags & 2) != 0, (flags & PNB_BWD_FP32_GEMM) == 0, L.part, part_floats(F) * sizeof(float), d_err, st, (flags & PNB_BWD_FP32_RECOMPUTE) != 0};
     PNB_REQUIRE(!cx.tc || d_err, PNB_ERR_INVALID, "pnb_shade_backward: the tensor-core path needs d_err");
     // ---------------- forward recompute ----------------
-    const bool pp = pts->rw2c != nullptr;                    // per-point frames
-    void (*build)(BwdParams) = F == PNB_FEAT ? (pp ? k_bwd_build<true, PNB_FEAT> : k_bwd_build<false, PNB_FEAT>)
-                                             : (pp ? k_bwd_build<true, PNB_FEAT_DTU> : k_bwd_build<false, PNB_FEAT_DTU>);
-    if (xs) build = k_bwd_build<false, PNB_FEAT_DTU, true>;
+    const auto build = with_frames(v, [](auto PP, auto F, auto XS) { return k_bwd_build<PP, F, XS>; });
     build<<<wb, 256, 0, st>>>(p);
     gemm_nn(cx, L.X1, KP1, mlp->w[0], 256, L.H1, 256, P, 256, KP1, mlp->b[0], 1);
     gemm_nn(cx, L.H1, 256, mlp->w[1], 256, L.X3, 272, P, 256, 256, mlp->b[1], 1);   // H2 into X3[:, :256]
@@ -720,10 +717,7 @@ extern "C" int pnb_shade_backward(const pnb_query_t* q, const pnb_points_t* pts,
     // dX1: only the 7F feature columns are consumed (k_bwd_scatter; no xyz gradient), rounded up to 16: 224 | 448
     gemm_nt(cx, L.G3, 256, mlp->w[0], 256, L.G1, KP1, P, (7 * F + 15) / 16 * 16, 256);
     // scatter to the points
-    void (*scatter)(BwdParams, const float*, float*, float*, float*, float*) =
-        F == PNB_FEAT ? (pp ? k_bwd_scatter<true, PNB_FEAT> : k_bwd_scatter<false, PNB_FEAT>)
-                      : (pp ? k_bwd_scatter<true, PNB_FEAT_DTU> : k_bwd_scatter<false, PNB_FEAT_DTU>);
-    if (xs) scatter = k_bwd_scatter<false, PNB_FEAT_DTU, true>;
+    const auto scatter = with_frames(v, [](auto PP, auto F, auto XS) { return k_bwd_scatter<PP, F, XS>; });
     scatter<<<(int)(((long)P * 4 + 255) / 256), 256, 0, st>>>(p, L.dwc, d_emb, d_color, d_dir, d_conf);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;

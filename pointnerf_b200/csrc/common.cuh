@@ -5,6 +5,10 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
+#include <type_traits>
+#include <vector>
+
 #include "../../include/pnb200.h"
 
 namespace pnb {
@@ -36,25 +40,72 @@ static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a
 static inline int feat_of(int32_t f) { return f == 0 ? PNB_FEAT : (f == PNB_FEAT || f == PNB_FEAT_DTU) ? (int)f : -1; }
 // block1.0 inputs [f (F), PE3(f) (6F), PE5(dists) (60)] = 7F + 60, padded to whole K = 32 blocks: 288 | 512
 __host__ __device__ constexpr int kpad1_of(int F) { return F == PNB_FEAT ? 288 : 512; }
-// The points' F (0 read as 32), which must have an instantiation and, with an MLP, equal the MLP's.  Sets the error text on failure.
-static inline int feat_check(const pnb_points_t* pts, const pnb_mlp_t* mlp, const char* fn, int* F) {
-    const int fp = feat_of(pts->feat_dim);
-    PNB_REQUIRE(fp > 0, PNB_ERR_UNSUPPORTED, "%s: point_features_dim %d unsupported (32 or 63)", fn, (int)pts->feat_dim);
-    if (mlp) {
-        const int fm = feat_of(mlp->feat_dim);
-        PNB_REQUIRE(fm == fp, PNB_ERR_INVALID, "%s: the MLP was built for point_features_dim %d, the points have %d", fn,
-                    (int)(mlp->feat_dim ? mlp->feat_dim : PNB_FEAT), fp);
+
+// ---- the run-time inputs that select a shading kernel's instantiation
+struct Variant {
+    int F;      // point_features_dim
+    bool pp;    // per-point frames (pts->rw2c != NULL)
+    bool xs;    // explicit samples (the frustum query, q->xs_loc_w != NULL)
+};
+// What an entry point requires of explicit samples
+enum class XsRule {
+    none,     // nothing (k_aux_outputs)
+    feat63,   // F = 63 (k_probe_outputs)
+    frames,   // F = 63, a uniform Rw2c and xs_loc / xs_dir given: the kernels that read the points' frames
+};
+// The points' F (0 read as 32), which must have an instantiation and, with an MLP, equal the MLP's; then explicit samples (q may be
+// NULL) by `rule`.  Sets the error text on failure.
+static inline int resolve_variant(const char* fn, const pnb_points_t* pts, const pnb_mlp_t* mlp, const pnb_query_t* q, XsRule rule,
+                                  Variant* v) {
+    const int F = feat_of(pts->feat_dim);
+    PNB_REQUIRE(F > 0, PNB_ERR_UNSUPPORTED, "%s: point_features_dim %d unsupported (32 or 63)", fn, (int)pts->feat_dim);
+    if (mlp)
+        PNB_REQUIRE(feat_of(mlp->feat_dim) == F, PNB_ERR_INVALID, "%s: the MLP was built for point_features_dim %d, the points have %d",
+                    fn, (int)(mlp->feat_dim ? mlp->feat_dim : PNB_FEAT), F);
+    *v = Variant{F, pts->rw2c != nullptr, q && q->xs_loc_w};
+    if (v->xs && rule == XsRule::frames) {
+        PNB_REQUIRE(q->xs_loc && q->xs_dir, PNB_ERR_INVALID, "%s: explicit samples need xs_loc_w, xs_loc and xs_dir", fn);
+        PNB_REQUIRE(F == PNB_FEAT_DTU && !v->pp, PNB_ERR_UNSUPPORTED,
+                    "%s: the frustum query's samples are shaded with point_features_dim 63 and a uniform Rw2c only", fn);
     }
-    *F = fp;
+    if (v->xs && rule == XsRule::feat63)
+        PNB_REQUIRE(F == PNB_FEAT_DTU, PNB_ERR_UNSUPPORTED, "%s: the frustum query's samples need point_features_dim 63", fn);
     return PNB_OK;
 }
-// Explicit samples (the frustum query, q->xs_loc_w set) are instantiated for the DTU scripts' configuration only: F = 63, one
-// uniform Rw2c, and all three geometry tensors given.  Sets the error text on failure.
-static inline int xs_check(const pnb_query_t* q, const pnb_points_t* pts, int F, const char* fn) {
-    if (!q->xs_loc_w) return PNB_OK;
-    PNB_REQUIRE(q->xs_loc && q->xs_dir, PNB_ERR_INVALID, "%s: explicit samples need xs_loc_w, xs_loc and xs_dir", fn);
-    PNB_REQUIRE(F == PNB_FEAT_DTU && !pts->rw2c, PNB_ERR_UNSUPPORTED,
-                "%s: the frustum query's samples are shaded with point_features_dim 63 and a uniform Rw2c only", fn);
+
+// ---- run-time values as template arguments.  Each helper calls f with std::integral_constant arguments, which convert to their
+// values in a template argument list, so that f names the instantiation: [](auto PP, auto F, auto XS) { return k<PP, F, XS>; }.
+// Only the combinations a helper passes are instantiated.
+template <bool B> using Bool = std::integral_constant<bool, B>;
+template <int I> using Int = std::integral_constant<int, I>;
+template <class Fn> static inline auto with_bool(bool b, Fn&& f) { return b ? f(Bool<true>{}) : f(Bool<false>{}); }
+template <class Fn> static inline auto with_feat(int F, Fn&& f) { return F == PNB_FEAT ? f(Int<PNB_FEAT>{}) : f(Int<PNB_FEAT_DTU>{}); }
+// f(F, XS) of k_probe_outputs: explicit samples at F = 63 only
+template <class Fn> static inline auto with_feat_xs(const Variant& v, Fn&& f) {
+    return v.xs ? f(Int<PNB_FEAT_DTU>{}, Bool<true>{}) : with_feat(v.F, [&](auto F) { return f(F, Bool<false>{}); });
+}
+// f(PP, F, XS) of the kernels that read the points' frames: explicit samples at F = 63 with a uniform Rw2c only
+template <class Fn> static inline auto with_frames(const Variant& v, Fn&& f) {
+    return v.xs ? f(Bool<false>{}, Int<PNB_FEAT_DTU>{}, Bool<true>{})
+                : with_bool(v.pp, [&](auto PP) { return with_feat(v.F, [&](auto F) { return f(PP, F, Bool<false>{}); }); });
+}
+
+// Prepares the launch of `kern` on the current device: opts it into `smem` bytes of dynamic shared memory the first time it is
+// launched there, and gives the device's SM count (n_sm may be NULL).  Call it for the selected kernel just before its launch.  The
+// state is per device, for one host thread per device.
+static inline int prepare_launch(const void* kern, size_t smem, int* n_sm, const char* fn) {
+    static std::vector<const void*> opted_in[64];
+    static int sm_count[64];
+    int dev = 0;
+    PNB_CHECK_CUDA(cudaGetDevice(&dev));
+    PNB_REQUIRE(dev >= 0 && dev < 64, PNB_ERR_UNSUPPORTED, "%s: device ordinal %d", fn, dev);
+    std::vector<const void*>& done = opted_in[dev];
+    if (std::find(done.begin(), done.end(), kern) == done.end()) {
+        PNB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        done.push_back(kern);
+    }
+    if (!sm_count[dev]) PNB_CHECK_CUDA(cudaDeviceGetAttribute(&sm_count[dev], cudaDevAttrMultiProcessorCount, dev));
+    if (n_sm) *n_sm = sm_count[dev];
     return PNB_OK;
 }
 

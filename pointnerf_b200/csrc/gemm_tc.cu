@@ -203,31 +203,23 @@ int gemm_tc(const GemmTc& g0, int splits, float* part_ws, size_t part_bytes, int
     PNB_REQUIRE(g.a_ks != 1 || g.a_rs % 4 == 0, PNB_ERR_INVALID, "gemm_tc: leading dimension of A must be a multiple of 4");
     PNB_REQUIRE(g.b_ks != 1 || g.b_rs % 4 == 0, PNB_ERR_INVALID, "gemm_tc: leading dimension of B must be a multiple of 4");
     PNB_REQUIRE(g.dact == nullptr || g.ldd % 2 == 0, PNB_ERR_INVALID, "gemm_tc: leading dimension of dact must be even");
-    static int configured[64] = {0};
-    int dev = 0;
-    PNB_CHECK_CUDA(cudaGetDevice(&dev));
     const bool precise = g.precise != 0;
     const size_t smem = (precise ? sizeof(gtc::Smem<3>) : sizeof(gtc::Smem<2>)) + 128;
     static_assert(sizeof(gtc::Smem<3>) + 128 <= 232448, "precise GEMM tile exceeds the shared memory of an SM");
-    if (dev >= 0 && dev < 64 && !configured[dev]) {
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_gemm_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(gtc::Smem<2>) + 128)));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_gemm_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(gtc::Smem<3>) + 128)));
-        configured[dev] = 1;
-    }
+    const auto kern = with_bool(precise, [](auto PRECISE) { return k_gemm_tc<PRECISE>; });
+    { const int rc = prepare_launch((const void*)kern, smem, nullptr, "gemm_tc"); if (rc) return rc; }
     if (splits <= 1) {
         g.kchunk = g.K; g.part = nullptr;
         dim3 grid((g.N + gtc::TN - 1) / gtc::TN, (g.M + gtc::TM - 1) / gtc::TM, 1);
         PNB_REQUIRE(!accumulate, PNB_ERR_INVALID, "gemm_tc: accumulation needs the split-K path");
-        if (precise) k_gemm_tc<true><<<grid, gtc::NTHR, smem, st>>>(g);
-        else k_gemm_tc<false><<<grid, gtc::NTHR, smem, st>>>(g);
+        kern<<<grid, gtc::NTHR, smem, st>>>(g);
     } else {
         int kchunk = ((g.K + splits - 1) / splits + 31) / 32 * 32;
         splits = (g.K + kchunk - 1) / kchunk;
         PNB_REQUIRE(part_ws && part_bytes >= (size_t)splits * g.M * g.N * sizeof(float), PNB_ERR_WORKSPACE, "gemm_tc: split-K workspace too small");
         g.kchunk = kchunk; g.part = part_ws;
         dim3 grid((g.N + gtc::TN - 1) / gtc::TN, (g.M + gtc::TM - 1) / gtc::TM, splits);
-        if (precise) k_gemm_tc<true><<<grid, gtc::NTHR, smem, st>>>(g);
-        else k_gemm_tc<false><<<grid, gtc::NTHR, smem, st>>>(g);
+        kern<<<grid, gtc::NTHR, smem, st>>>(g);
         const long n = (long)g.M * g.N;
         k_splitk_reduce<<<(int)((n + 255) / 256), 256, 0, st>>>(part_ws, splits, g.M, g.N, g.C, g.ldc, accumulate);
     }

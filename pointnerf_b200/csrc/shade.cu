@@ -542,29 +542,13 @@ extern "C" int pnb_shade_forward(const pnb_query_t* q, const pnb_points_t* pts, 
     PNB_REQUIRE(q->K >= 1 && q->K <= PNB_MAX_K, PNB_ERR_UNSUPPORTED, "pnb_shade_forward: K=%d unsupported", q->K);
     for (int i = 0; i < 9; ++i)
         PNB_REQUIRE(mlp->w[i] && mlp->b[i], PNB_ERR_INVALID, "pnb_shade_forward: MLP tensor %d is null", i);
-    int F = 0;
-    { const int rc = feat_check(pts, mlp, "pnb_shade_forward", &F); if (rc) return rc; }
-    const bool xs = q->xs_loc_w != nullptr;
-    { const int rc = xs_check(q, pts, F, "pnb_shade_forward"); if (rc) return rc; }
-    static int smem_set[64] = {0}, n_sm_of[64] = {0};      // per device of this process
-    int dev = 0;
-    PNB_CHECK_CUDA(cudaGetDevice(&dev));
-    PNB_REQUIRE(dev >= 0 && dev < 64, PNB_ERR_UNSUPPORTED, "pnb_shade_forward: device ordinal %d", dev);
-    if (!smem_set[dev]) {
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false, PNB_FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true, PNB_FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false, PNB_FEAT_DTU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<true, PNB_FEAT_DTU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_shade_fwd<false, PNB_FEAT_DTU, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ShadeSmem)));
-        PNB_CHECK_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
-        smem_set[dev] = 1;
-    }
-    const int n_sm = n_sm_of[dev];
+    Variant v;
+    { const int rc = resolve_variant("pnb_shade_forward", pts, mlp, q, XsRule::frames, &v); if (rc) return rc; }
     ShadeParams p;
     p.q = *q; p.pts = *pts; p.mlp = *mlp; p.o = *opts; p.sigma_rgb = (float4*)d_sigma_rgb;
-    void (*kern)(ShadeParams) = F == PNB_FEAT ? (pts->rw2c ? k_shade_fwd<true, PNB_FEAT> : k_shade_fwd<false, PNB_FEAT>)
-                                              : (pts->rw2c ? k_shade_fwd<true, PNB_FEAT_DTU> : k_shade_fwd<false, PNB_FEAT_DTU>);
-    if (xs) kern = k_shade_fwd<false, PNB_FEAT_DTU, true>;
+    const auto kern = with_frames(v, [](auto PP, auto F, auto XS) { return k_shade_fwd<PP, F, XS>; });
+    int n_sm = 0;
+    { const int rc = prepare_launch((const void*)kern, sizeof(ShadeSmem), &n_sm, "pnb_shade_forward"); if (rc) return rc; }
     kern<<<n_sm, NTHREADS, sizeof(ShadeSmem), stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
@@ -575,9 +559,9 @@ static int composite(const pnb_query_t* q, const pnb_shade_opts_t* opts, const f
     CompositeParams p;
     p.q = *q; p.o = *opts; p.sigma_rgb = (const float4*)d_sigma_rgb;
     p.ray_color = d_ray_color; p.opacity = d_opacity; p.bg_T = d_bg_T; p.ray_mask = d_ray_mask; p.bg_ray = d_bg_ray;
-    const bool xs = q->xs_loc_w != nullptr;
-    void (*kern)(CompositeParams) = d_bg_ray ? (xs ? k_composite<true, true> : k_composite<false, true>)
-                                             : (xs ? k_composite<true, false> : k_composite<false, false>);
+    const auto kern = with_bool(q->xs_loc_w != nullptr, [&](auto XS) {
+        return with_bool(d_bg_ray != nullptr, [&](auto BGR) { return k_composite<XS, BGR>; });
+    });
     kern<<<(q->R + 127) / 128, 128, 0, stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
@@ -602,16 +586,16 @@ extern "C" int pnb_aux_outputs(const pnb_query_t* q, const pnb_points_t* pts, co
     cudaStream_t stream = (cudaStream_t)stream_;
     PNB_REQUIRE(q && pts && d_opacity && d_weight && d_conf_coefficient && d_blend_weight, PNB_ERR_INVALID, "pnb_aux_outputs: null argument");
     PNB_REQUIRE(q->K >= 1 && q->K <= PNB_MAX_K, PNB_ERR_UNSUPPORTED, "pnb_aux_outputs: K=%d unsupported", q->K);
-    int F = 0;
-    { const int rc = feat_check(pts, nullptr, "pnb_aux_outputs", &F); if (rc) return rc; }
+    Variant v;
+    { const int rc = resolve_variant("pnb_aux_outputs", pts, nullptr, q, XsRule::none, &v); if (rc) return rc; }
     if (n_rows <= 0) return PNB_OK;
     PNB_REQUIRE(d_rows, PNB_ERR_INVALID, "pnb_aux_outputs: null row list");
     AuxParams p;
     p.q = *q; p.xyz = pts->xyz; p.conf = pts->conf; p.rows = d_rows; p.n_rows = n_rows; p.opacity = d_opacity;
     p.weight = d_weight; p.cc = d_conf_coefficient; p.blend = d_blend_weight; p.grad_cc = nullptr; p.grad_conf = nullptr;
     const long long n = (long long)n_rows * q->SR;
-    if (q->xs_loc_w) k_aux_outputs<true><<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(p);
-    else k_aux_outputs<false><<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(p);
+    const auto kern = with_bool(v.xs, [](auto XS) { return k_aux_outputs<XS>; });
+    kern<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }
@@ -624,8 +608,8 @@ extern "C" int pnb_probe_outputs(const pnb_query_t* q, const pnb_points_t* pts, 
                 PNB_ERR_INVALID, "pnb_probe_outputs: null argument");
     PNB_REQUIRE(q->K >= 1 && q->K <= PNB_MAX_K, PNB_ERR_UNSUPPORTED, "pnb_probe_outputs: K=%d unsupported", q->K);
     PNB_REQUIRE(q->SR >= 1 && q->SR <= PNB_MAX_SR, PNB_ERR_UNSUPPORTED, "pnb_probe_outputs: SR=%d unsupported (1..%d)", q->SR, PNB_MAX_SR);
-    int F = 0;
-    { const int rc = feat_check(pts, nullptr, "pnb_probe_outputs", &F); if (rc) return rc; }
+    Variant v;     // the check on explicit samples runs only when there are rows to launch for
+    { const int rc = resolve_variant("pnb_probe_outputs", pts, nullptr, q, n_rows > 0 ? XsRule::feat63 : XsRule::none, &v); if (rc) return rc; }
     PNB_REQUIRE(d_rows || n_rows == q->R, PNB_ERR_INVALID, "pnb_probe_outputs: without a row list n_rows must be R (%d), got %d", q->R, n_rows);
     if (n_rows <= 0) return PNB_OK;
     ProbeParams p;
@@ -633,11 +617,8 @@ extern "C" int pnb_probe_outputs(const pnb_query_t* q, const pnb_points_t* pts, 
     p.max_opacity = d_max_opacity; p.max_loc = d_max_loc; p.far_dist = d_far_dist; p.avg_color = d_avg_color; p.avg_dir = d_avg_dir;
     p.avg_conf = d_avg_conf; p.avg_emb = d_avg_emb; p.slot = d_slot; p.weight = d_weight;
     const unsigned blocks = (unsigned)((n_rows + 3) / 4);   // 4 rays (warps) per block
-    if (q->xs_loc_w) {
-        PNB_REQUIRE(F == PNB_FEAT_DTU, PNB_ERR_UNSUPPORTED, "pnb_probe_outputs: the frustum query's samples need point_features_dim 63");
-        k_probe_outputs<PNB_FEAT_DTU, true><<<blocks, 128, 0, stream>>>(p);
-    } else if (F == PNB_FEAT) k_probe_outputs<PNB_FEAT><<<blocks, 128, 0, stream>>>(p);
-    else k_probe_outputs<PNB_FEAT_DTU><<<blocks, 128, 0, stream>>>(p);
+    const auto kern = with_feat_xs(v, [](auto F, auto XS) { return k_probe_outputs<F, XS>; });
+    kern<<<blocks, 128, 0, stream>>>(p);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }

@@ -474,10 +474,11 @@ __device__ __forceinline__ QuadRow quad_row(uint32_t head, int tot, int lane) {
 // pre[n][c] = b1[c] + sum_{k<7F} W1^T[k][c] * x_n[k],  x_n = [f (F), PE3(f) (6F, column F + 6*feature + 2*j + {sin, cos})]: the
 // point-only inputs of block1.0 (F = 32: exactly the first 7 K blocks of the operand build_pair_part writes).  fp32 FMAs in ascending k.
 // Block = NP points x 256 columns (F = 63: 16 points, the 441 inputs padded to 444 with zeros).
+__host__ __device__ constexpr int point_pre_np(int F) { return F == PNB_FEAT ? 32 : 16; }   // points per block
 template <int F>
 __global__ void __launch_bounds__(256) k_point_pre(const float* __restrict__ emb, int N, const float* __restrict__ w1t, const float* __restrict__ b1,
                                                    float* __restrict__ pre) {
-    constexpr int NP = F == PNB_FEAT ? 32 : 16;           // points per block
+    constexpr int NP = point_pre_np(F);
     constexpr int KX = (7 * F + 3) / 4 * 4;               // inputs, whole float4: 224 | 444
     __shared__ __align__(16) float x[NP][KX + 4];
     const int n0 = blockIdx.x * NP;
@@ -995,10 +996,11 @@ extern "C" int pnb_point_pre(const pnb_points_t* pts, const pnb_mlp_t* mlp, floa
     cudaStream_t stream = (cudaStream_t)stream_;
     PNB_REQUIRE(pts && mlp && d_pre, PNB_ERR_INVALID, "pnb_point_pre: null argument");
     PNB_REQUIRE(pre_bytes >= pnb_point_pre_bytes(pts->N), PNB_ERR_WORKSPACE, "pnb_point_pre: buffer too small");
-    int F = 0;
-    { const int rc = feat_check(pts, mlp, "pnb_point_pre", &F); if (rc) return rc; }
-    if (pts->N > 0 && F == PNB_FEAT) k_point_pre<PNB_FEAT><<<(pts->N + 31) / 32, 256, 0, stream>>>(pts->emb, pts->N, mlp->w[0], mlp->b[0], d_pre);
-    else if (pts->N > 0) k_point_pre<PNB_FEAT_DTU><<<(pts->N + 15) / 16, 256, 0, stream>>>(pts->emb, pts->N, mlp->w[0], mlp->b[0], d_pre);
+    Variant v;
+    { const int rc = resolve_variant("pnb_point_pre", pts, mlp, nullptr, XsRule::none, &v); if (rc) return rc; }
+    const int np = point_pre_np(v.F);
+    const auto kern = with_feat(v.F, [](auto F) { return k_point_pre<F>; });
+    if (pts->N > 0) kern<<<(pts->N + np - 1) / np, 256, 0, stream>>>(pts->emb, pts->N, mlp->w[0], mlp->b[0], d_pre);
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
 }
@@ -1055,40 +1057,15 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
     PNB_REQUIRE(ws_bytes >= pnb_shade_tc_bytes(max_valid_samples), PNB_ERR_WORKSPACE, "pnb_shade_forward_tc: workspace too small");
     const bool frozen = (flags & PNB_TC_FROZEN) != 0;
     PNB_REQUIRE(!frozen || d_point_pre, PNB_ERR_INVALID, "pnb_shade_forward_tc: PNB_TC_FROZEN needs the table of pnb_point_pre");
-    int F = 0;
-    { const int rc = feat_check(pts, mlp, "pnb_shade_forward_tc", &F); if (rc) return rc; }
-    const bool xs = q->xs_loc_w != nullptr;                  // explicit samples (the frustum query)
-    { const int rc = xs_check(q, pts, F, "pnb_shade_forward_tc"); if (rc) return rc; }
-    static int configured[64] = {0}, n_sm_of[64] = {0};      // per device of this process (one process per GPU is the norm)
-    int dev = 0;
-    PNB_CHECK_CUDA(cudaGetDevice(&dev));
-    PNB_REQUIRE(dev >= 0 && dev < 64, PNB_ERR_UNSUPPORTED, "pnb_shade_forward_tc: device ordinal %d", dev);
+    Variant v;
+    { const int rc = resolve_variant("pnb_shade_forward_tc", pts, mlp, q, XsRule::frames, &v); if (rc) return rc; }
     // interleaved (non-swizzled) operand layout: 128-byte alignment of the carve-out is sufficient
     constexpr size_t kSmemMax = 232448;   // 227 KB opt-in limit per block on sm_90
     const size_t smem_pair = sizeof(hw::Smem) + 128, smem_color = sizeof(hcw::Smem) + 128;
     static_assert(sizeof(hw::Smem) + 128 <= kSmemMax, "pair kernel shared-memory carve-out exceeds the per-block limit");
     static_assert(sizeof(hcw::Smem) + 128 <= kSmemMax, "colour kernel shared-memory carve-out exceeds the per-block limit");
-    if (!configured[dev]) {
-        const void* pair_kernels[20] = {
-            (const void*)k_shade_wg<false, false, false, PNB_FEAT>, (const void*)k_shade_wg<false, true, false, PNB_FEAT>,
-            (const void*)k_shade_wg<true, false, false, PNB_FEAT>, (const void*)k_shade_wg<true, true, false, PNB_FEAT>,
-            (const void*)k_shade_wg<false, false, true, PNB_FEAT>, (const void*)k_shade_wg<false, true, true, PNB_FEAT>,
-            (const void*)k_shade_wg<true, false, true, PNB_FEAT>, (const void*)k_shade_wg<true, true, true, PNB_FEAT>,
-            (const void*)k_shade_wg<false, false, false, PNB_FEAT_DTU>, (const void*)k_shade_wg<false, true, false, PNB_FEAT_DTU>,
-            (const void*)k_shade_wg<true, false, false, PNB_FEAT_DTU>, (const void*)k_shade_wg<true, true, false, PNB_FEAT_DTU>,
-            (const void*)k_shade_wg<false, false, true, PNB_FEAT_DTU>, (const void*)k_shade_wg<false, true, true, PNB_FEAT_DTU>,
-            (const void*)k_shade_wg<true, false, true, PNB_FEAT_DTU>, (const void*)k_shade_wg<true, true, true, PNB_FEAT_DTU>,
-            (const void*)k_shade_wg<false, false, false, PNB_FEAT_DTU, true>, (const void*)k_shade_wg<false, true, false, PNB_FEAT_DTU, true>,
-            (const void*)k_shade_wg<true, false, false, PNB_FEAT_DTU, true>, (const void*)k_shade_wg<true, true, false, PNB_FEAT_DTU, true>};
-        for (const void* k : pair_kernels) PNB_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pair));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
-        PNB_CHECK_CUDA(cudaFuncSetAttribute(k_color_wg<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_color));
-        PNB_CHECK_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
-        configured[dev] = 1;
-    }
     // PNB_TC_FEW_CTAS (test of the persistent tile loop): one CTA per 8 SMs, so every CTA runs many tiles
-    const int n_cta = (flags & PNB_TC_FEW_CTAS) ? (n_sm_of[dev] + 7) / 8 : n_sm_of[dev];
+    const auto ctas = [flags](int n_sm) { return (flags & PNB_TC_FEW_CTAS) ? (n_sm + 7) / 8 : n_sm; };
     TcWs w(ws, ws_bytes, max_valid_samples);
     ShadeTcParams p;
     p.q = *q; p.pts = *pts; p.o = *opts; p.wimg = (const unsigned char*)d_packed;
@@ -1099,36 +1076,30 @@ extern "C" int pnb_shade_forward_tc(const pnb_query_t* q, const pnb_points_t* pt
     p.vcnt = w.vcntp; p.vorder = w.vorder; p.quad_first = w.quad_first; p.pack_cnt = w.pack_cnt;
     p.pre = d_point_pre;
     if (flags & PNB_TC_PAIRS) {
+        const auto kern = with_bool(frozen, [&](auto FROZEN) {
+            return with_bool(opts->agg_intrp_order == 1, [&](auto O1) {
+                return with_frames(v, [&](auto PP, auto F, auto XS) { return k_shade_wg<FROZEN, O1, PP, F, XS>; });
+            });
+        });
+        int n_sm = 0;
+        { const int rc = prepare_launch((const void*)kern, smem_pair, &n_sm, "pnb_shade_forward_tc"); if (rc) return rc; }
         const int cap = max_valid_samples, n_sc = (int)pack_sc_max(cap);
         k_pack_quads<<<(n_sc + 7) / 8, 256, 0, stream>>>(p.q, cap, w.sc_quads, w.quad_local, w.vorder, w.vcntp, (float4*)d_sigma_rgb);
         k_pack_scan<<<1, 1024, 0, stream>>>(p.q, cap, w.sc_quads, w.quad_first, w.pack_cnt);
         k_pack_place<<<(cap + 255) / 256, 256, 0, stream>>>(p.q, cap, w.sc_quads, w.quad_local, w.quad_first);
-        const bool o1 = opts->agg_intrp_order == 1;              // compile-time flags of the kernel
-        const bool pp = pts->rw2c != nullptr;
-        void (*kern)(ShadeTcParams) =
-            F == PNB_FEAT ? (frozen ? (o1 ? (pp ? k_shade_wg<true, true, true, PNB_FEAT> : k_shade_wg<true, true, false, PNB_FEAT>)
-                                          : (pp ? k_shade_wg<true, false, true, PNB_FEAT> : k_shade_wg<true, false, false, PNB_FEAT>))
-                                    : (o1 ? (pp ? k_shade_wg<false, true, true, PNB_FEAT> : k_shade_wg<false, true, false, PNB_FEAT>)
-                                          : (pp ? k_shade_wg<false, false, true, PNB_FEAT> : k_shade_wg<false, false, false, PNB_FEAT>)))
-                          : (frozen ? (o1 ? (pp ? k_shade_wg<true, true, true, PNB_FEAT_DTU> : k_shade_wg<true, true, false, PNB_FEAT_DTU>)
-                                          : (pp ? k_shade_wg<true, false, true, PNB_FEAT_DTU> : k_shade_wg<true, false, false, PNB_FEAT_DTU>))
-                                    : (o1 ? (pp ? k_shade_wg<false, true, true, PNB_FEAT_DTU> : k_shade_wg<false, true, false, PNB_FEAT_DTU>)
-                                          : (pp ? k_shade_wg<false, false, true, PNB_FEAT_DTU> : k_shade_wg<false, false, false, PNB_FEAT_DTU>)));
-        if (xs)
-            kern = frozen ? (o1 ? k_shade_wg<true, true, false, PNB_FEAT_DTU, true> : k_shade_wg<true, false, false, PNB_FEAT_DTU, true>)
-                          : (o1 ? k_shade_wg<false, true, false, PNB_FEAT_DTU, true> : k_shade_wg<false, false, false, PNB_FEAT_DTU, true>);
-        kern<<<n_cta, hw::NTHR_CTA, smem_pair, stream>>>(p);
+        kern<<<ctas(n_sm), hw::NTHR_CTA, smem_pair, stream>>>(p);
     }
     if (flags & PNB_TC_COLOR) {
         ColorTcParams ct;
-        ct.q = *q; ct.o = *opts; ct.wimg = (const unsigned char*)d_packed + pack_pairs_bytes(F);
+        ct.q = *q; ct.o = *opts; ct.wimg = (const unsigned char*)d_packed + pack_pairs_bytes(v.F);
         for (int i = 0; i < 3; ++i) ct.bias[i] = mlp->b[5 + i];
         ct.w3t = mlp->w[8]; ct.b3 = mlp->b[8];
         ct.hbar = w.hbar; ct.sigma = w.sigma; ct.hbar_cap = max_valid_samples; ct.sigma_rgb = (float4*)d_sigma_rgb; ct.err = d_err;
         ct.pts = *pts;
-        if (xs) k_color_wg<false, true><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
-        else if (pts->rw2c) k_color_wg<true><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
-        else k_color_wg<false><<<n_cta, hcw::NTHR_CTA, smem_color, stream>>>(ct);
+        const auto kern = with_frames(v, [](auto PP, auto F, auto XS) { return k_color_wg<PP, XS>; });
+        int n_sm = 0;
+        { const int rc = prepare_launch((const void*)kern, smem_color, &n_sm, "pnb_shade_forward_tc"); if (rc) return rc; }
+        kern<<<ctas(n_sm), hcw::NTHR_CTA, smem_color, stream>>>(ct);
     }
     PNB_CHECK_CUDA(cudaGetLastError());
     return PNB_OK;
