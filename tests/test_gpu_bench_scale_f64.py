@@ -13,10 +13,12 @@ A. The training step (bench.py train_section: `train` on ship_optimise, N = 600k
    scale, every other row of the 600k or 5M must be exactly zero, bit for bit, the 18 MLP tensors to RTOL, points_conf of point 0 to
    grad_check.point0_conf_bound, and the loss to float64; no outlier allowance.  Scattered rays spread every point's atomic adds over
    many tiles, and scannet's touched points lie above 2^22.  Neither bench step reaches the split-K cap of the dW GEMMs (64 slabs of
-   2048 pair rows), so scannet's first two batches also run as one step, which does.
+   2048 pair rows), so scannet's first two batches also run as one step, which does.  Ship also runs with F = 63 (bench_feat63.py's
+   training leg: point_features_dim 63, point modes 01) in modes 0, 4 and 1 on the same batch.
 B. The forward, sample by sample (tests/test_gpu_forward_f64.py's `_run` and its table), on seeded sets of 1024 pixels over the whole
    truck_8gpu, scannet_8gpu and lego_render frames, with the frozen, general and fp32 kernels; truck adds the image-corner strip of
-   tests/test_gpu_shade.py.  Every row of the frozen cloud's `pre` table is compared with float64, in row chunks.
+   tests/test_gpu_shade.py.  lego_render also runs with F = 63 (bench_feat63.py's render leg) and with scene.edit_frames' per-point
+   frames (bench_rw2c.py).  Every row of the frozen cloud's `pre` table is compared with float64, in row chunks.
 C. The whole frame (runner.render_image, as the bench renders it) equals render_full on B's pixel subset bit for bit, which equals
    forward()'s result on its hit rays: B's float64 check covers the frame the bench renders.
 
@@ -200,25 +202,31 @@ def bench_batch(cfg, batches=1):
     return kw, torch.cat(gt), rays
 
 
-# (config, pnb_bwd_fp32 mode, pnb_precision, bench batches in the step).  The bench's scannet step has ~106k pair rows (51.6 slabs of
-# 2048), below the split-K cap of the tensor-core dW GEMMs (64 slabs, csrc/backward.cu SPLITK_MAX); its first two batches as one step
-# (~211k rows) run the pair layers' dW GEMMs with the cap, every slab taller than 2048 rows.
-TRAIN_CASES = [("ship_optimise", 0, "bf16x3", 1), ("ship_optimise", 4, "bf16x3", 1), ("ship_optimise", 1, "bf16x3", 1),
-               ("ship_optimise", 1, "fp32", 1),
-               ("scannet_8gpu", 0, "bf16x3", 1), ("scannet_8gpu", 4, "bf16x3", 1), ("scannet_8gpu", 1, "bf16x3", 1),
-               ("scannet_8gpu", 0, "bf16x3", 2), ("scannet_8gpu", 4, "bf16x3", 2)]
+# (config, pnb_bwd_fp32 mode, pnb_precision, bench batches in the step, point_features_dim F).  The bench's scannet step has ~106k pair
+# rows (51.6 slabs of 2048), below the split-K cap of the tensor-core dW GEMMs (64 slabs, csrc/backward.cu SPLITK_MAX); its first two
+# batches as one step (~211k rows) run the pair layers' dW GEMMs with the cap, every slab taller than 2048 rows.  F = 63 on ship is
+# bench_feat63.bench_train's 63-channel leg (the DTU scripts' point_features_dim 63, point modes 01) on the same batches.
+TRAIN_CASES = [("ship_optimise", 0, "bf16x3", 1, 32), ("ship_optimise", 4, "bf16x3", 1, 32), ("ship_optimise", 1, "bf16x3", 1, 32),
+               ("ship_optimise", 1, "fp32", 1, 32),
+               ("scannet_8gpu", 0, "bf16x3", 1, 32), ("scannet_8gpu", 4, "bf16x3", 1, 32), ("scannet_8gpu", 1, "bf16x3", 1, 32),
+               ("scannet_8gpu", 0, "bf16x3", 2, 32), ("scannet_8gpu", 4, "bf16x3", 2, 32),
+               ("ship_optimise", 0, "bf16x3", 1, 63), ("ship_optimise", 4, "bf16x3", 1, 63), ("ship_optimise", 1, "bf16x3", 1, 63)]
 
 
-@pytest.mark.parametrize("cfg_name,mode,precision,batches", TRAIN_CASES, ids=["%s-mode%d-%s-x%d" % c for c in TRAIN_CASES])
-def test_training_step_gradients(cfg_name, mode, precision, batches):
+def _train_id(c):
+    return "%s-mode%d-%s-x%d" % c[:4] + ("" if c[4] == 32 else "-F%d" % c[4])
+
+
+@pytest.mark.parametrize("cfg_name,mode,precision,batches,F", TRAIN_CASES, ids=[_train_id(c) for c in TRAIN_CASES])
+def test_training_step_gradients(cfg_name, mode, precision, batches, F):
     with _device_released():
-        _training_step_case(cfg_name, mode, precision, batches)
+        _training_step_case(cfg_name, mode, precision, batches, F)
 
 
-def _training_step_case(cfg_name, mode, precision, batches):
+def _training_step_case(cfg_name, mode, precision, batches, F=32):
     cfg = scene.CONFIGS[cfg_name]
     _reset_peak_memory()
-    net, _, opt = harness.build_model(cfg, DEV, alpha_bias=3.0, is_train=True, pnb_precision=precision, pnb_bwd_fp32=mode)
+    net, _, opt = harness.build_model(cfg, DEV, alpha_bias=3.0, is_train=True, pnb_precision=precision, pnb_bwd_fp32=mode, feat_dim=F)
     ts = parallel.TrainStep(net, world=1)
     kw, gt, rays = bench_batch(cfg, batches)
     n_rays = batches * BATCH
@@ -229,7 +237,7 @@ def _training_step_case(cfg_name, mode, precision, batches):
     N = npn.xyz.shape[0]
     q = net.last
     cam = rays["camrotc2w"][0]
-    slopes, ex, P = grad_check.kernel_masks(net, q, 32, cam)
+    slopes, ex, P = grad_check.kernel_masks(net, q, F, cam)
     slopes = [s == 1 for s in slopes]         # 1 byte per unit instead of 8; _slopes rebuilds the same values per chunk
     peak = torch.cuda.max_memory_allocated(DEV)
     pidx, loc_w = ex["sample_pidx"].cpu(), ex["sample_loc_w"].cpu()
@@ -256,9 +264,9 @@ def _training_step_case(cfg_name, mode, precision, batches):
     max_idx = int(keep.max())
     del net, npn, ts, got, q, kw, ex      # the next case gets the device without this one's 5M rows
     torch.cuda.empty_cache()
-    print("\n[bench-f64] train %s mode=%d %s x%d: N=%d R'=%d of %d (hit %.3f) P=%d (%.1f x 2048) U=%d max point %d, empty slots %d (n0=%d) "
+    print("\n[bench-f64] train %s F=%d mode=%d %s x%d: N=%d R'=%d of %d (hit %.3f) P=%d (%.1f x 2048) U=%d max point %d, empty slots %d (n0=%d) "
           "peak %.2f GB oracle %.0f s | points=%.2e (%s) mlp=%.2e (%s, %d tensors) conf0=%.2e/%.2e untouched=%s loss=%.9f |d|=%.2e/%.2e" % (
-              cfg_name, mode, precision, batches, N, Rn, n_rays, Rn / n_rays, P, P / 2048, keep.numel(), max_idx, n_empty, n0, peak / 1e9, t_oracle,
+              cfg_name, F, mode, precision, batches, N, Rn, n_rays, Rn / n_rays, P, P / 2048, keep.numel(), max_idx, n_empty, n0, peak / 1e9, t_oracle,
               max(err[k] for k in pts_keys), max(pts_keys, key=err.get), max(err[k] for k in mlp_keys), max(mlp_keys, key=err.get),
               len(mlp_keys), conf0[0], conf0[1], untouched, loss, d_loss, b_loss))
     assert len(mlp_keys) == 18
@@ -322,13 +330,27 @@ def test_forward_over_the_whole_frame(cfg_name, kernel, monkeypatch):
         _frame_case(cfg_name, kernel)
 
 
-def _frame_case(cfg_name, kernel):
+# the other bench lines on lego_render: bench_feat63.bench_render's 63-channel frame (F 63), bench_rw2c's per-point frames
+# (scene.edit_frames, as test_gpu_forward_f64._run(frames=True) forms them)
+LEGS = {"F63": dict(F=63), "rw2c": dict(frames=True)}
+
+
+@pytest.mark.parametrize("kernel", ["frozen", "general", "fp32"])
+@pytest.mark.parametrize("leg", list(LEGS))
+def test_forward_over_the_whole_frame_bench_legs(leg, kernel, monkeypatch):
+    """test_forward_over_the_whole_frame on lego_render for the bench_feat63 and bench_rw2c legs."""
+    monkeypatch.setattr(fwd, "_pre_errors", _pre_errors_in_chunks)
+    with _device_released():
+        _frame_case("lego_render", kernel, **LEGS[leg])
+
+
+def _frame_case(cfg_name, kernel, F=32, frames=False):
     cfg = scene.CONFIGS[cfg_name]
     pixels = frame_pixels(cfg)
     if cfg_name == "truck_8gpu":
         pixels = np.concatenate([pixels, _block(*TRUCK_CORNER)])
     _reset_peak_memory()
-    net, sh, smap = fwd._run(cfg_name, F=32, kernel=kernel, rotated=False, pixels=pixels)
+    net, sh, smap = fwd._run(cfg_name, F=F, kernel=kernel, frames=frames, rotated=False, pixels=pixels)
     hit, rays, out = smap["hit"], smap["rays"], smap["out"]
     pidx = smap["sample_pidx"]
     max_idx = int(pidx.max())
@@ -347,8 +369,8 @@ def _frame_case(cfg_name, kernel):
     peak = torch.cuda.max_memory_allocated(DEV)
     del net, sub, img, out, smap
     torch.cuda.empty_cache()
-    print("[bench-f64] frame %s %s: %d pixels, %d hit; frame %dx%d, %d hit; max point %d; peak %.2f GB; subset == forward %s; "
-          "frame == subset %s" % (cfg_name, kernel, pixels.shape[0], int(hit.sum()), cfg.W, cfg.H, n_frame_hit, max_idx, peak / 1e9,
+    print("[bench-f64] frame %s F=%d frames=%s %s: %d pixels, %d hit; frame %dx%d, %d hit; max point %d; peak %.2f GB; subset == forward %s; "
+          "frame == subset %s" % (cfg_name, F, frames, kernel, pixels.shape[0], int(hit.sum()), cfg.W, cfg.H, n_frame_hit, max_idx, peak / 1e9,
                                   same_sub, same_frame))
     assert all(same_sub.values()), "render_full on the subset differs from forward(): %s" % same_sub
     assert all(same_frame.values()), "the whole frame differs from render_full on its pixels: %s" % same_frame
