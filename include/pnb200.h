@@ -417,6 +417,34 @@ int pnb_plane_bg(const float* d_xyz, int R, int G, const float* d_w2c, const flo
                  const long long* d_mask_off, const int8_t* d_masks, const float* d_img, int H, int W, const float* d_plane_color,
                  float* d_bg, pnb_stream_t stream);
 
+/* ---- depth filter and visual hull of the initial point cloud ----
+ * Replaces filter_utils.filter_by_masks_gpu (models/mvs/filter_utils.py:157-291, manual_depth_view 1) and mvs_utils.alpha_masking
+ * (models/mvs/mvs_utils.py:573-607) for pointnerf_b200.depth_filter.  Every fp32 operation is rounded explicitly in the order
+ * csrc/depth_filter.cu documents (DESIGN.md §5 "Depth filter and visual hull").
+ * Views (V of them, all H x W): d_depth [V,H,W] fp32 (the depth maps), d_K [V,3,3], d_Kinv [V,3,3], d_c2w [V,3,4] (rows 0..2 of the
+ * inverse extrinsics), d_pair [V,V,3,4] (pair (r, s): rows 0..2 of E_s inv(E_r)).  A call filters the nr ref views r0 .. r0+nr-1;
+ * d_conf, d_mask and d_xyz are device arrays of nr device pointers, one per ref view: its confidence [H,W] fp32, points mask [H,W]
+ * (nonzero bytes are true) and camera points [H,W,3] fp32 (raw x, y; the depth is read from d_depth). */
+size_t pnb_depth_filter_bytes(int nr, int H, int W);
+/* The geometric-consistency test of every pixel of the nr ref views against every other view, the averaged depth, the confidence /
+ * mask / geo_cnsst_num decision and, with d_ranges (device float[6], lo then hi; NULL: none), the inclusive range test on the world
+ * point.  Synchronises the stream once, to return the number of kept points of every ref view in h_counts (int64 [nr]).  ws must
+ * outlive pnb_depth_filter_outputs on it. */
+int pnb_depth_filter_build(void* ws, size_t ws_bytes, int V, int H, int W, int r0, int nr, const float* d_depth,
+                           const float* const* d_conf, const uint8_t* const* d_mask, const float* const* d_xyz, const float* d_K,
+                           const float* d_Kinv, const float* d_c2w, const float* d_pair, const float* d_ranges, float conf_thresh,
+                           int geo_cnsst_num, pnb_stream_t stream, long long* h_counts);
+/* The kept points of a pnb_depth_filter_build, ref view after ref view, each in row-major pixel order: d_xyz_cam [n,3] (raw x, y and
+ * the averaged depth), d_xyz_world [n,3], d_conf_out [n] (n: the sum of h_counts).  Nothing synchronises. */
+int pnb_depth_filter_outputs(const void* ws, size_t ws_bytes, int H, int W, int r0, int nr, const float* const* d_xyz,
+                             const float* const* d_conf, const float* d_c2w, float* d_xyz_cam, float* d_xyz_world, float* d_conf_out,
+                             pnb_stream_t stream);
+/* Visual-hull mask d_mask [N] (bytes 0 / 1) of the points d_points [N,3] fp32 over V views: d_w2c [V,3,4] (rows 0..2), d_K [V,3,3],
+ * d_alpha [V,H,W] fp32.  h_near_far (host float[2]: near - 1 and far, already rounded to fp32; NULL: no depth test); range_test != 0
+ * adds 1 to the alpha of a point whose pixel is outside the image.  Nothing synchronises. */
+int pnb_alpha_mask(const float* d_points, long long N, int V, const float* d_w2c, const float* d_K, const float* d_alpha, int H, int W,
+                   const float* h_near_far, int range_test, uint8_t* d_mask, pnb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

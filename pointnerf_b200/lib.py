@@ -79,7 +79,8 @@ SYMBOLS = ["pnb_version", "pnb_last_error", "pnb_struct_size", "pnb_grid_bytes",
            "pnb_shade_tc_tables", "pnb_shade_tc_buffers", "pnb_backward_bytes", "pnb_shade_backward", "pnb_backward_tables", "pnb_aux_outputs",
            "pnb_aux_conf_backward", "pnb_probe_outputs", "pnb_frustum_bytes", "pnb_frustum_build", "pnb_frustum_query_bytes", "pnb_frustum_query",
            "pnb_frustum_export", "pnb_frustum_samples_bytes", "pnb_frustum_samples", "pnb_composite_forward_bg_ray",
-           "pnb_vox_bytes", "pnb_vox_build", "pnb_vox_outputs", "pnb_plane_cross", "pnb_plane_fg_masks", "pnb_plane_bg"]
+           "pnb_vox_bytes", "pnb_vox_build", "pnb_vox_outputs", "pnb_plane_cross", "pnb_plane_fg_masks", "pnb_plane_bg",
+           "pnb_depth_filter_bytes", "pnb_depth_filter_build", "pnb_depth_filter_outputs", "pnb_alpha_mask"]
 # test-only library (csrc/selftest/pnb200_selftest.h)
 SELFTEST_LIB_PATH = os.path.join(_HERE, "csrc", "libpnb200_selftest.so")
 SELFTEST_SYMBOLS = ["pnb_selftest_last_error", "pnb_umma_selftest", "pnb_umma_selftest2", "pnb_gemm_tc_test"]
@@ -201,6 +202,16 @@ def load():
     lib.pnb_plane_fg_masks.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
     lib.pnb_plane_bg.restype = C.c_int
     lib.pnb_plane_bg.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int] + [C.c_void_p] * 3
+    lib.pnb_depth_filter_bytes.restype = C.c_size_t
+    lib.pnb_depth_filter_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+    lib.pnb_depth_filter_build.restype = C.c_int
+    lib.pnb_depth_filter_build.argtypes = [C.c_void_p, C.c_size_t] + [C.c_int] * 5 + [C.c_void_p] * 9 + [C.c_float, C.c_int, C.c_void_p,
+                                                                                                          C.POINTER(C.c_longlong)]
+    lib.pnb_depth_filter_outputs.restype = C.c_int
+    lib.pnb_depth_filter_outputs.argtypes = [C.c_void_p, C.c_size_t] + [C.c_int] * 4 + [C.c_void_p] * 7
+    lib.pnb_alpha_mask.restype = C.c_int
+    lib.pnb_alpha_mask.argtypes = [C.c_void_p, C.c_longlong, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int, C.POINTER(C.c_float), C.c_int,
+                                                                                         C.c_void_p, C.c_void_p]
     _lib = lib
     return lib
 
